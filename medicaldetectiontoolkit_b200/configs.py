@@ -11,8 +11,8 @@ def _retina_scales(base):
 
 
 def make_cf(model='retina_unet', dim=3, patch_size=(128, 128, 128), exp='lidc_exp', batch_size=2):
-    """model in {'retina_unet', 'retina_net', 'mrcnn', 'detection_unet'}; exp in {'lidc_exp', 'toy_exp'} selects the filter widths (and the
-    Detection U-Net's n_roi_candidates)."""
+    """model in {'retina_unet', 'retina_net', 'mrcnn', 'ufrcnn', 'detection_unet'}; exp in {'lidc_exp', 'toy_exp'} selects the filter widths,
+    the Detection U-Net's n_roi_candidates and UFRCNN+'s sampling sizes, roi_chunk_size and learning-rate schedule length."""
     cf = types.SimpleNamespace()
     cf.dim = dim
     cf.model = model
@@ -86,6 +86,21 @@ def make_cf(model='retina_unet', dim=3, patch_size=(128, 128, 128), exp='lidc_ex
         cf.operate_stride1 = (model == 'retina_unet')
     else:
         cf.n_anchors_per_pos = len(cf.rpn_anchor_ratios)
+    if model == 'ufrcnn':
+        # add_mrcnn_configs + the `ufrcnn` block of experiments/{lidc_exp,toy_exp}/configs.py, including the values that differ by experiment
+        # or dim there and that the other models here take from the lidc_exp 3D config
+        cf.operate_stride1 = True
+        cf.class_specific_seg_flag = True
+        cf.num_seg_classes = 3
+        cf.frcnn_mode = True
+        cf.return_masks_in_test = False
+        cf.n_plot_rpn_props = 5 if dim == 2 else 30
+        if exp == 'toy_exp':
+            cf.learning_rate = [1e-4] * 24
+            cf.rpn_train_anchors_per_image = 2
+            cf.train_rois_per_image = 2
+            if dim == 2:
+                cf.roi_chunk_size = 800
     if model == 'detection_unet':
         # add_det_unet_configs of experiments/{lidc_exp,toy_exp}/configs.py
         cf.aggregation_operation = 'max'

@@ -203,7 +203,9 @@ def pyramid_roi_align(feature_maps, rois, pool_size, pyramid_levels, dim):
 
 
 def detection_target_layer(batch_proposals, batch_mrcnn_class_scores, batch_gt_class_ids, batch_gt_boxes, batch_gt_masks, cf):
-    """sample positive / SHEM-negative rois per batch element and build their class, box and mask targets (mrcnn.py:461-613)"""
+    """sample positive / SHEM-negative rois per batch element and build their class, box and mask targets (mrcnn.py:461-613).
+    batch_gt_masks None: no mask targets (UFRCNN+'s variant, ufrcnn.py:461-587); the fourth result is then None."""
+    with_masks = batch_gt_masks is not None
     dev = batch_proposals.device
     dim = cf.dim
     scale = torch.as_tensor(np.asarray(cf.scale), dtype=torch.float32, device=dev)
@@ -218,7 +220,8 @@ def detection_target_layer(batch_proposals, batch_mrcnn_class_scores, batch_gt_c
         positive_samples = 0
         if has_gt:
             gt_boxes = torch.as_tensor(np.asarray(batch_gt_boxes[b])).float().to(dev) / scale
-            gt_masks = torch.as_tensor(np.asarray(batch_gt_masks[b])).float().to(dev)      # (n_gt, y, x, (z), c)
+            if with_masks:
+                gt_masks = torch.as_tensor(np.asarray(batch_gt_masks[b])).float().to(dev)  # (n_gt, y, x, (z), c)
             overlaps = mutils.bbox_overlaps(proposals, gt_boxes)
             roi_iou_max = overlaps.max(dim=1)[0]
             positive_idx = torch.nonzero(roi_iou_max >= (0.5 if dim == 2 else 0.3)).squeeze(1)
@@ -230,13 +233,13 @@ def detection_target_layer(batch_proposals, batch_mrcnn_class_scores, batch_gt_c
                 positive_rois = proposals[positive_idx]
                 assign = overlaps[positive_idx].max(dim=1)[1]
                 deltas = mutils.box_refinement(positive_rois, gt_boxes[assign]) / torch.as_tensor(cf.bbox_std_dev, dtype=torch.float32, device=dev)
-                roi_masks = gt_masks[assign][..., 0]
-                box_ids = torch.arange(roi_masks.shape[0], device=dev).int()
-                fn = ra2D(cf.mask_shape[0], cf.mask_shape[1], 0) if dim == 2 else ra3D(cf.mask_shape[0], cf.mask_shape[1], cf.mask_shape[2], 0)
-                masks = torch.round(fn(roi_masks.unsqueeze(1).contiguous(), positive_rois, box_ids).squeeze(1))
+                if with_masks:
+                    roi_masks = gt_masks[assign][..., 0]
+                    box_ids = torch.arange(roi_masks.shape[0], device=dev).int()
+                    fn = ra2D(cf.mask_shape[0], cf.mask_shape[1], 0) if dim == 2 else ra3D(cf.mask_shape[0], cf.mask_shape[1], cf.mask_shape[2], 0)
+                    masks_l.append(torch.round(fn(roi_masks.unsqueeze(1).contiguous(), positive_rois, box_ids).squeeze(1)))
                 pos_ix.append(element_ix[positive_idx])
                 deltas_l.append(deltas)
-                masks_l.append(masks)
                 cls_l.append(gt_class_ids[assign])
                 positive_count += positive_samples
         else:
@@ -251,11 +254,11 @@ def detection_target_layer(batch_proposals, batch_mrcnn_class_scores, batch_gt_c
     parts_ix = pos_ix + neg_ix
     if not parts_ix:
         return (torch.zeros(0, dtype=torch.long, device=dev), torch.zeros(0, dtype=torch.int32, device=dev),
-                torch.zeros((0, dim * 2), device=dev), torch.zeros((0,) + mask_shape, device=dev))
+                torch.zeros((0, dim * 2), device=dev), torch.zeros((0,) + mask_shape, device=dev) if with_masks else None)
     sample_indices = torch.cat(parts_ix)
     target_class_ids = torch.cat(cls_l + [torch.zeros(negative_count, dtype=torch.int32, device=dev)])
     target_deltas = torch.cat(deltas_l + [torch.zeros((negative_count, dim * 2), device=dev)])
-    target_masks = torch.cat(masks_l + [torch.zeros((negative_count,) + mask_shape, device=dev)])
+    target_masks = torch.cat(masks_l + [torch.zeros((negative_count,) + mask_shape, device=dev)]) if with_masks else None
     return sample_indices, target_class_ids, target_deltas, target_masks
 
 
