@@ -10,13 +10,11 @@ keys and results_dict format):
 """
 import numpy as np
 import torch
-import torch.nn as nn
 
-from . import model_utils as mutils
 from . import native_ops
+from ._detector import Detector
 from .backbone import FPN
 from .conv import NDConvGenerator, no_split_consumer
-from .retina_unet import net as _retina_net
 
 
 def _box_lists(boxes, scores, n_kept, n_fg):
@@ -34,32 +32,13 @@ def _box_lists(boxes, scores, n_kept, n_fg):
     return out_coords, out_scores
 
 
-class net(nn.Module):
+class net(Detector):
 
-    def __init__(self, cf, logger=None):
-        super().__init__()
-        self.cf = cf
-        self.logger = logger
+    def build(self):
+        cf = self.cf
         conv = NDConvGenerator(cf.dim)
         self.fpn = FPN(cf, conv, operate_stride1=True)
         self.conv_final = no_split_consumer(conv(cf.end_filts, cf.num_seg_classes, ks=1, pad=0, norm=cf.norm, relu=None))
-        if getattr(cf, 'weight_init', None) is not None:
-            if logger is not None:
-                logger.info("using pytorch weight init of type {}".format(cf.weight_init))
-            mutils.initialize_weights(self)
-        elif logger is not None:
-            logger.info("using default pytorch weight init")
-
-    _to_host = _retina_net._to_host
-
-    def _to_device(self, arr, dtype=torch.float32):
-        dev = next(self.parameters()).device
-        if torch.is_tensor(arr):
-            return arr.to(dev, dtype=dtype, non_blocking=True)
-        t = torch.from_numpy(np.ascontiguousarray(arr))
-        if dev.type == 'cuda':
-            t = t.pin_memory()
-        return t.to(dev, non_blocking=True).to(dtype)
 
     def _logits(self, x):
         return self.conv_final(self.fpn(x)[0])

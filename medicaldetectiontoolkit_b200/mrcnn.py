@@ -9,8 +9,10 @@ load key-for-key).
   pyramid_roi_align                       :373-457         csrc/roi_align.cu (channels-last, 128-bit gathers / vector atomics in backward)
   detection_target_layer                  :461-613         broadcast IoU, RoIAlign on GT masks, device SHEM
   refine_detections                       :620-714         one batched multi-class NMS launch (groups translated apart), top-k per element
-  numpy gt_anchor_matching per element    :894             fp64 device kernels (csrc/anchor_match.cu)
+  numpy gt_anchor_matching per element    :894             fp64 device kernels (csrc/anchor_match.cu) on a side stream
 """
+import functools
+
 import numpy as np
 import scipy.ndimage
 import torch
@@ -19,6 +21,7 @@ import torch.nn.functional as F
 
 from . import model_utils as mutils
 from . import native_ops
+from ._detector import Detector, anchor_losses, append_anchor_boxes, match_anchors
 from .backbone import FPN
 from .conv import Conv3d, NDConvGenerator, _Conv3dFn, no_split_consumer
 from .native_ops import CropAndResizeFunction as ra3D, CropAndResizeFunction2D as ra2D
@@ -317,10 +320,11 @@ def _unmold_mask(mask, box, spatial):
     return out
 
 
-def get_results(cf, img_shape, detections, detection_masks, box_results_list=None, return_masks=True):
-    """results_dict {'boxes', 'seg_preds'} (mrcnn.py:717-799)"""
+def get_results(cf, img_shape, detections, detection_masks, box_results_list=None, return_masks=True, host=None):
+    """results_dict {'boxes', 'seg_preds'} (mrcnn.py:717-799).
+    host: optional detections as a numpy array already copied to the host (train_forward batches its device->host copies)"""
     dim = cf.dim
-    det = detections.detach().cpu().numpy()
+    det = detections.detach().cpu().numpy() if host is None else host
     masks_np = detection_masks.detach().movedim(1, -1).cpu().numpy() if return_masks else None
     if box_results_list is None:
         box_results_list = [[] for _ in range(img_shape[0])]
@@ -347,73 +351,63 @@ def get_results(cf, img_shape, detections, detection_masks, box_results_list=Non
     return {'boxes': box_results_list, 'seg_preds': np.round(np.array(seg_preds))[:, np.newaxis].astype('uint8')}
 
 
-# ------------------------------------------------------------------------------------------------------------------ net
-class net(nn.Module):
+def first_stage(net, fmaps, is_training):
+    """RPN on every pyramid level, proposals and the gradient-free classifier pass over all proposals in roi_chunk_size chunks (mrcnn.py:
+    987-1036).  Sets net.mrcnn_feature_maps, net.rpn_rois_batch_info and net.batch_mrcnn_class_scores for loss_samples_forward.
+    -> (rpn_pred_logits, rpn_pred_deltas, batch_proposal_boxes, arguments of refine_detections without cf)"""
+    cf = net.cf
+    net.mrcnn_feature_maps = fmaps
+    outs = list(zip(*[net.rpn(p) for p in fmaps]))
+    rpn_pred_logits, rpn_pred_probs, rpn_pred_deltas = [torch.cat(list(o), dim=1) for o in outs]
+    proposal_count = cf.post_nms_rois_training if is_training else cf.post_nms_rois_inference
+    with torch.no_grad():
+        batch_rpn_rois, batch_proposal_boxes = proposal_layer(rpn_pred_probs.detach(), rpn_pred_deltas.detach(), proposal_count, net.anchors, cf)
+        b, P = batch_rpn_rois.shape[0], batch_rpn_rois.shape[1]
+        batch_ixs = torch.arange(b, device=batch_rpn_rois.device).repeat_interleave(P).float()
+        rpn_rois = batch_rpn_rois.view(-1, batch_rpn_rois.shape[2])
+        net.rpn_rois_batch_info = torch.cat((rpn_rois, batch_ixs.unsqueeze(1)), dim=1)
+        logits_l, bbox_l = [], []
+        for chunk in net.rpn_rois_batch_info.split(cf.roi_chunk_size):
+            cl, bb = net.classifier(fmaps, chunk)
+            logits_l.append(cl)
+            bbox_l.append(bb)
+        net.batch_mrcnn_class_scores = F.softmax(torch.cat(logits_l, 0), dim=1)
+    return rpn_pred_logits, rpn_pred_deltas, batch_proposal_boxes, (rpn_rois, net.batch_mrcnn_class_scores, torch.cat(bbox_l, 0), batch_ixs)
 
-    def __init__(self, cf, logger=None):
-        super().__init__()
-        self.cf = cf
-        self.logger = logger
-        self.build()
-        if getattr(cf, 'weight_init', None) is not None:
-            if logger is not None:
-                logger.info("using pytorch weight init of type {}".format(cf.weight_init))
-            mutils.initialize_weights(self)                       # mrcnn.py:819-823
-        elif logger is not None:
-            logger.info("using default pytorch weight init")
+
+def append_proposal_boxes(host_props, host_rois, host_t_cls, cf, box_results_list):
+    """the top n_plot_rpn_props proposals of each element and the second stage's positive / negative samples for the monitoring plots
+    (mrcnn.py:904-916), from host copies of the proposals, the window-clipped sampled rois and their target class ids"""
+    for b, props in enumerate(host_props):
+        for r in props[props[:, -1].argsort()][::-1][:cf.n_plot_rpn_props, :-1]:
+            box_results_list[b].append({'box_coords': r, 'box_type': 'prop'})
+    for ix, r in enumerate(host_rois):
+        box_results_list[int(r[-1])].append({'box_coords': r[:-1] * cf.scale, 'box_type': 'pos_class' if host_t_cls[ix] > 0 else 'neg_class'})
+
+
+# ------------------------------------------------------------------------------------------------------------------ net
+class net(Detector):
 
     def build(self):
         cf = self.cf
-        h, w = cf.patch_size[:2]
-        if h / 2 ** 5 != int(h / 2 ** 5) or w / 2 ** 5 != int(w / 2 ** 5):
-            raise Exception("Image size must be dividable by 2 at least 5 times to avoid fractions when downscaling and upscaling.")
-        if len(cf.patch_size) == 3:
-            d = cf.patch_size[2]
-            if d / 2 ** 3 != int(d / 2 ** 3):
-                raise Exception("Image z dimension must be dividable by 2 at least 3 times to avoid fractions when downscaling and upscaling.")
+        self._check_patch_size(check_z=True)
         conv = NDConvGenerator(cf.dim)
-        self.np_anchors = mutils.generate_pyramid_anchors(self.logger, cf)
-        self.register_buffer("anchors", torch.from_numpy(self.np_anchors).float(), persistent=False)
-        self.register_buffer("anchors_f64", torch.from_numpy(self.np_anchors).double(), persistent=False)
+        self._register_anchors()
         self.fpn = FPN(cf, conv, operate_stride1=False)
         self.rpn = RPN(cf, conv)
         self.classifier = Classifier(cf, conv)
         self.mask = Mask(cf, conv)
 
-    def _to_device(self, arr, dtype=torch.float32):
-        dev = self.anchors.device
-        if torch.is_tensor(arr):
-            return arr.to(dev, dtype=dtype, non_blocking=True)
-        t = torch.from_numpy(np.ascontiguousarray(arr))
-        if dev.type == 'cuda':
-            t = t.pin_memory()
-        return t.to(dev, non_blocking=True).to(dtype)
-
     def forward(self, img, is_training=True):
         """-> [rpn_pred_logits, rpn_pred_deltas, batch_proposal_boxes, detections, detection_masks] (mrcnn.py:987-1049)"""
         cf = self.cf
         fpn_outs = self.fpn(img)
-        fmaps = [fpn_outs[i] for i in cf.pyramid_levels]
-        self.mrcnn_feature_maps = fmaps
-        outs = list(zip(*[self.rpn(p) for p in fmaps]))
-        rpn_pred_logits, rpn_pred_probs, rpn_pred_deltas = [torch.cat(list(o), dim=1) for o in outs]
-        proposal_count = cf.post_nms_rois_training if is_training else cf.post_nms_rois_inference
+        rpn_pred_logits, rpn_pred_deltas, batch_proposal_boxes, refine_args = first_stage(self, [fpn_outs[i] for i in cf.pyramid_levels], is_training)
         with torch.no_grad():
-            batch_rpn_rois, batch_proposal_boxes = proposal_layer(rpn_pred_probs.detach(), rpn_pred_deltas.detach(), proposal_count, self.anchors, cf)
-            b, P = batch_rpn_rois.shape[0], batch_rpn_rois.shape[1]
-            batch_ixs = torch.arange(b, device=img.device).repeat_interleave(P).float()
-            rpn_rois = batch_rpn_rois.view(-1, batch_rpn_rois.shape[2])
-            self.rpn_rois_batch_info = torch.cat((rpn_rois, batch_ixs.unsqueeze(1)), dim=1)
-            logits_l, bbox_l = [], []
-            for chunk in self.rpn_rois_batch_info.split(cf.roi_chunk_size):
-                cl, bb = self.classifier(fmaps, chunk)
-                logits_l.append(cl)
-                bbox_l.append(bb)
-            self.batch_mrcnn_class_scores = F.softmax(torch.cat(logits_l, 0), dim=1)
-            detections = refine_detections(rpn_rois, self.batch_mrcnn_class_scores, torch.cat(bbox_l, 0), batch_ixs, cf)
+            detections = refine_detections(*refine_args, cf)
             sp = list(img.shape[2:])
             scale = torch.as_tensor([sp[0], sp[1], sp[0], sp[1]] + ([sp[2], sp[2]] if cf.dim == 3 else []) + [1], dtype=torch.float32, device=img.device)
-            detection_masks = self.mask(fmaps, detections[:, :cf.dim * 2 + 1] / scale)
+            detection_masks = self.mask(self.mrcnn_feature_maps, detections[:, :cf.dim * 2 + 1] / scale)
         return [rpn_pred_logits, rpn_pred_deltas, batch_proposal_boxes, detections, detection_masks]
 
     def loss_samples_forward(self, batch_gt_class_ids, batch_gt_boxes, batch_gt_masks):
@@ -431,71 +425,45 @@ class net(nn.Module):
         return [logits, boxes, mask, t_cls, t_deltas, t_mask, sample_proposals]
 
     def train_forward(self, batch, is_validation=False, **kwargs):
+        """batch {'data', 'seg', 'bb_target', 'roi_labels', 'roi_masks'} -> results_dict {'boxes', 'seg_preds', 'torch_loss', 'monitor_values',
+        'logger_string'} (mrcnn.py:853-966).  The RPN matching (and its host waits) runs first on a side stream; the network and every loss
+        are then queued; the detections, loss values, sample classes and monitoring boxes come back in one batched device->host copy."""
         cf = self.cf
         gt_class_ids, gt_boxes = batch['roi_labels'], batch['bb_target']
         axes = (0, 2, 3, 1) if cf.dim == 2 else (0, 2, 3, 4, 1)
         gt_masks = [np.transpose(batch['roi_masks'][ii], axes=axes) for ii in range(len(batch['roi_masks']))]
         img = self._to_device(batch['data'])
-        n_b = img.shape[0]
-        box_results_list = [[] for _ in range(n_b)]
-        # the RPN matching needs only the GT boxes: run it (and its host synchronisation) before the network is queued
-        matched = []
-        for b in range(n_b):
-            if len(gt_boxes[b]) > 0:
-                for ix in range(len(gt_boxes[b])):
-                    box_results_list[b].append({'box_coords': gt_boxes[b][ix], 'box_label': gt_class_ids[b][ix], 'box_type': 'gt'})
-                matched.append(mutils.gt_anchor_matching_device(cf, self.anchors_f64, gt_boxes[b], return_pos=True))   # class-agnostic
-            else:
-                matched.append((torch.full((self.anchors.shape[0],), -1, dtype=torch.int32, device=img.device),
-                                torch.zeros((cf.rpn_train_anchors_per_image, 2 * cf.dim), dtype=torch.float64, device=img.device),
-                                torch.zeros(0, dtype=torch.long, device=img.device)))
+        box_results_list = [[] for _ in range(img.shape[0])]
+        matched = match_anchors(self, gt_boxes, gt_class_ids, box_results_list, img.device, class_agnostic=True)
         rpn_class_logits, rpn_pred_deltas, proposal_boxes, detections, detection_masks = self.forward(img)
         logits, pred_deltas, pred_mask, t_cls, t_deltas, t_mask, sample_proposals = self.loss_samples_forward(gt_class_ids, gt_boxes, gt_masks)
-
-        max_pos = max(1, cf.rpn_train_anchors_per_image // 2)
-        rpn_class_loss = img.new_zeros(1)
-        rpn_bbox_loss = img.new_zeros(1)
-        monitor = []
-        for b, (rpn_match, rpn_target_deltas, pos_ids) in enumerate(matched):
-            cl, neg_ix = compute_rpn_class_loss(rpn_match, rpn_class_logits[b], cf.shem_poolsize, max_pos=max_pos, pos_ids=pos_ids)
-            monitor.append((rpn_match, neg_ix))
-            rpn_class_loss = rpn_class_loss + cl / n_b
-            rpn_bbox_loss = rpn_bbox_loss + compute_rpn_bbox_loss(rpn_target_deltas, rpn_pred_deltas[b], rpn_match, max_pos=max_pos, pos_ids=pos_ids) / n_b
-        if kwargs.get('monitor_anchors', True):
-            # positive / sampled-negative anchors of the RPN loss for the monitoring plots (mrcnn.py:896-916)
-            sp = img.shape[2:]
-            hi = np.array([sp[0], sp[1], sp[0], sp[1]] + ([sp[2], sp[2]] if cf.dim == 3 else []))
-            for b, (match, neg_ix) in enumerate(monitor):
-                m = match.cpu().numpy()
-                neg_all = np.where(m == -1)[0]
-                nix = neg_ix.cpu().numpy()
-                for p_ in np.clip(self.np_anchors[m == 1], 0, hi):
-                    box_results_list[b].append({'box_coords': p_, 'box_type': 'pos_anchor'})
-                if neg_all.size:
-                    for n_ in np.clip(self.np_anchors[neg_all[nix[nix >= 0]]], 0, hi):
-                        box_results_list[b].append({'box_coords': n_, 'box_type': 'neg_anchor'})
-            props = proposal_boxes.cpu().numpy()
-            for b in range(n_b):
-                for r in props[b][props[b][:, -1].argsort()][::-1][:cf.n_plot_rpn_props, :-1]:
-                    box_results_list[b].append({'box_coords': r, 'box_type': 'prop'})
-            if sample_proposals.shape[0] > 0:
-                rois = mutils.clip_to_window(cf.window, sample_proposals.clone()).cpu().numpy()
-                tc = t_cls.cpu().numpy()
-                for ix, r in enumerate(rois):
-                    box_results_list[int(r[-1])].append({'box_coords': r[:-1] * cf.scale, 'box_type': 'pos_class' if tc[ix] > 0 else 'neg_class'})
-
+        rpn_class_loss, rpn_bbox_loss, monitor = anchor_losses(matched, rpn_class_logits, rpn_pred_deltas, cf,
+                                                               functools.partial(compute_rpn_class_loss, shem_poolsize=cf.shem_poolsize),
+                                                               compute_rpn_bbox_loss)
         mrcnn_class_loss = compute_mrcnn_class_loss(t_cls, logits)
         mrcnn_bbox_loss = compute_mrcnn_bbox_loss(t_deltas, pred_deltas, t_cls)
         mrcnn_mask_loss = compute_mrcnn_mask_loss(t_mask, pred_mask, t_cls) if not cf.frcnn_mode else img.new_zeros(())
         loss = rpn_class_loss + rpn_bbox_loss + mrcnn_class_loss + mrcnn_bbox_loss + mrcnn_mask_loss
+
+        vals = torch.stack([v.detach().reshape(()) for v in (loss, rpn_class_loss, rpn_bbox_loss, mrcnn_class_loss, mrcnn_bbox_loss, mrcnn_mask_loss)])
+        dcount = torch.stack([(t_cls == c).sum() for c in range(1, cf.head_classes)])
+        show = kwargs.get('monitor_anchors', True)
+        to_host = [detections, vals, dcount]
+        if show:
+            to_host += [t_cls, proposal_boxes, mutils.clip_to_window(cf.window, sample_proposals.clone())] + [t for pair in monitor for t in pair]
+        host = self._to_host(to_host)
+        if show:
+            # positive / sampled-negative anchors of the RPN loss, top proposals and the second-stage samples (mrcnn.py:896-916)
+            append_anchor_boxes(self.np_anchors, host[6::2], host[7::2], img.shape[2:], cf.dim, box_results_list)
+            append_proposal_boxes(host[4], host[5], host[3], cf, box_results_list)
+
         return_masks = cf.return_masks_in_val if is_validation else False
-        results_dict = get_results(cf, img.shape, detections, detection_masks, box_results_list, return_masks=return_masks)
+        results_dict = get_results(cf, img.shape, detections, detection_masks, box_results_list, return_masks=return_masks, host=host[0])
         results_dict['torch_loss'] = loss
-        vals = torch.stack([v.detach().reshape(()) for v in (loss, rpn_class_loss, rpn_bbox_loss, mrcnn_class_loss, mrcnn_bbox_loss, mrcnn_mask_loss)]).cpu().tolist()
-        dcount = [int((t_cls == c).sum().item()) for c in range(1, cf.head_classes)]
+        vals = host[1].tolist()
         results_dict['monitor_values'] = {'loss': vals[0], 'class_loss': vals[3]}
         results_dict['logger_string'] = "loss: {0:.2f}, rpn_class: {1:.2f}, rpn_bbox: {2:.2f}, mrcnn_class: {3:.2f}, mrcnn_bbox: {4:.2f}, " \
-                                        "mrcnn_mask: {5:.2f}, dcount {6}".format(*vals, dcount)
+                                        "mrcnn_mask: {5:.2f}, dcount {6}".format(*vals, host[2].tolist())
         return results_dict
 
     def test_forward(self, batch, return_masks=True):

@@ -10,8 +10,6 @@ results_dict keys), re-designed so that a training step never leaves the GPU:
   refine_detections                    :194-271                 top-k instead of a 5.4 M-element sort; ONE batched multi-class NMS launch
   nms_3D per (batch, class) + D2H mask pth_nms.py / nms_cuda.c  csrc/nms.cu bitmask + on-device reduction
 """
-import contextlib
-
 import numpy as np
 import torch
 import torch.nn as nn
@@ -19,6 +17,7 @@ import torch.nn.functional as F
 
 from . import model_utils as mutils
 from . import native_ops
+from ._detector import Detector, anchor_losses, append_anchor_boxes, match_anchors, seg_loss_terms
 from .backbone import FPN
 from .conv import NDConvGenerator, no_split_consumer
 
@@ -245,45 +244,17 @@ def get_results(cf, img_shape, detections, seg_logits, box_results_list=None, ho
     return results
 
 
-_SIDE_STREAMS = {}
-_PINNED = {}      # pinned device->host staging buffers of train_forward, keyed by (net, slot, shape, dtype)
-
-
-def _side_stream(dev):
-    """one side stream per device for the GT<->anchor matching (kept out of the module so that nets stay picklable / deep-copyable)"""
-    key = (dev.type, dev.index)
-    if key not in _SIDE_STREAMS:
-        _SIDE_STREAMS[key] = torch.cuda.Stream(device=dev)
-    return _SIDE_STREAMS[key]
-
-
 # ------------------------------------------------------------------------------------------------------------------ net
-class net(nn.Module):
+class net(Detector):
     """Retina U-Net.  `operate_stride1`/seg head follow cf (set cf.operate_stride1 False and num_seg_classes 0 for plain RetinaNet)."""
 
     has_seg_head = True
 
-    def __init__(self, cf, logger=None):
-        super().__init__()
-        self.cf = cf
-        self.logger = logger
-        self.build()
-        if getattr(cf, 'weight_init', None) is not None:
-            if logger is not None:
-                logger.info("using pytorch weight init of type {}".format(cf.weight_init))
-            mutils.initialize_weights(self)                       # retina_unet.py:360-364
-        elif logger is not None:
-            logger.info("using default pytorch weight init")
-
     def build(self):
         cf = self.cf
-        h, w = cf.patch_size[:2]
-        if h / 2 ** 5 != int(h / 2 ** 5) or w / 2 ** 5 != int(w / 2 ** 5):
-            raise Exception("Image size must be dividable by 2 at least 5 times to avoid fractions when downscaling and upscaling.")
+        self._check_patch_size()
         conv = NDConvGenerator(cf.dim)
-        self.np_anchors = mutils.generate_pyramid_anchors(self.logger, cf)
-        self.register_buffer("anchors", torch.from_numpy(self.np_anchors).float(), persistent=False)
-        self.register_buffer("anchors_f64", torch.from_numpy(self.np_anchors).double(), persistent=False)
+        self._register_anchors()
         self.Fpn = FPN(cf, conv, operate_stride1=cf.operate_stride1)
         self.Classifier = Classifier(cf, conv)
         self.BBRegressor = BBRegressor(cf, conv)
@@ -318,32 +289,6 @@ class net(nn.Module):
             flat_softmax = F.softmax(class_logits.detach().view(-1, class_logits.shape[-1]), 1)
             return refine_detections(self.anchors, flat_softmax, bb_outputs.detach().view(-1, bb_outputs.shape[-1]), batch_ixs, self.cf)
 
-    def _to_host(self, tensors):
-        """device tensors -> numpy through cached pinned staging buffers: all copies are queued, then ONE synchronisation"""
-        outs = []
-        for i, t in enumerate(tensors):
-            t = t.detach().contiguous()
-            key = (id(self), i, tuple(t.shape), t.dtype)
-            buf = _PINNED.get(key)
-            if buf is None:
-                buf = torch.empty(t.shape, dtype=t.dtype, pin_memory=t.is_cuda)
-                _PINNED[key] = buf
-            buf.copy_(t, non_blocking=True)
-            outs.append(buf)
-        if tensors and tensors[0].is_cuda:
-            torch.cuda.current_stream(tensors[0].device).synchronize()
-        return [o.numpy().copy() for o in outs]
-
-    def _to_device(self, arr, dtype=torch.float32):
-        """host batch array -> device through pinned memory (non_blocking H2D)"""
-        dev = self.anchors.device
-        if torch.is_tensor(arr):
-            return arr.to(dev, dtype=dtype, non_blocking=True)
-        t = torch.from_numpy(np.ascontiguousarray(arr))
-        if dev.type == 'cuda':
-            t = t.pin_memory()
-        return t.to(dev, non_blocking=True).to(dtype)
-
     def train_forward(self, batch, **kwargs):
         """batch: {'data', 'seg', 'bb_target', 'roi_labels', ...} numpy -> results_dict with 'torch_loss', 'boxes', 'seg_preds',
         'monitor_values', 'logger_string' (retina_unet.py:381-456).
@@ -352,62 +297,16 @@ class net(nn.Module):
         (and its host synchronisation) runs first; backbone, heads and all losses are then queued without a sync; the detections for the
         monitoring output (NMS, variable-length result) and every device->host copy come last and share one synchronisation."""
         cf = self.cf
-        gt_class_ids = batch['roi_labels']
-        gt_boxes = batch['bb_target']
         img = self._to_device(batch['data'])
-        n_b = img.shape[0]
-        dev = img.device
-        box_results_list = [[] for _ in range(n_b)]
-        seg = None
-        if self.has_seg_head:
-            fused_seg = FUSED_LOSSES and img.is_cuda and cf.num_seg_classes <= 8
-            seg = self._to_device(batch['seg'], dtype=torch.uint8 if fused_seg else torch.long)   # (b, 1, y, x, (z)); uint8: 1 byte per voxel over PCIe
-
-        # The matching synchronises with the host (exact-length positive lists, numpy sub-sampling).  On a side stream those waits cover only the
-        # matching kernels, so the host is not held up by — and the GPU not drained of — the previous step's backward pass still in flight.
-        main_stream = torch.cuda.current_stream(dev) if img.is_cuda else None
-        match_stream = _side_stream(dev) if main_stream is not None else None
-        matched = []
-        with (torch.cuda.stream(match_stream) if main_stream is not None else contextlib.nullcontext()):
-            for b in range(n_b):
-                if len(gt_boxes[b]) > 0:
-                    for ix in range(len(gt_boxes[b])):
-                        box_results_list[b].append({'box_coords': batch['bb_target'][b][ix], 'box_label': batch['roi_labels'][b][ix], 'box_type': 'gt'})
-                    matched.append(mutils.gt_anchor_matching_device(cf, self.anchors_f64, gt_boxes[b], gt_class_ids[b], return_pos=True))
-                else:
-                    matched.append((torch.full((self.anchors.shape[0],), -1, dtype=torch.int32, device=dev),
-                                    torch.zeros((cf.rpn_train_anchors_per_image, 2 * cf.dim), dtype=torch.float64, device=dev),
-                                    torch.zeros(0, dtype=torch.long, device=dev)))
-        if main_stream is not None:
-            main_stream.wait_stream(match_stream)              # the losses (main stream) consume the matching's tensors
-            for tup in matched:
-                for t in tup:
-                    t.record_stream(main_stream)
+        box_results_list = [[] for _ in range(img.shape[0])]
+        seg = self._seg_to_device(batch['seg'], FUSED_LOSSES) if self.has_seg_head else None
+        matched = match_anchors(self, batch['bb_target'], batch['roi_labels'], box_results_list, img.device)
 
         class_logits, pred_deltas, seg_logits = self._forward_logits(img)
-
-        max_pos = max(1, cf.rpn_train_anchors_per_image // 2)
-        batch_class_loss = img.new_zeros(1)
-        batch_bbox_loss = img.new_zeros(1)
-        monitor = []
-        for b, (match, target_deltas, pos_ids) in enumerate(matched):
-            class_loss, neg_ix = compute_class_loss(match, class_logits[b], max_pos=max_pos, pos_ids=pos_ids)
-            bbox_loss = compute_bbox_loss(target_deltas, pred_deltas[b], match, max_pos=max_pos, pos_ids=pos_ids)
-            batch_class_loss = batch_class_loss + class_loss / n_b
-            batch_bbox_loss = batch_bbox_loss + bbox_loss / n_b
-            monitor.append((match, neg_ix))
-
+        batch_class_loss, batch_bbox_loss, monitor = anchor_losses(matched, class_logits, pred_deltas, cf, compute_class_loss, compute_bbox_loss)
         loss = batch_class_loss + batch_bbox_loss
-        seg_dice = seg_ce = None
         if self.has_seg_head:
-            if fused_seg:
-                # one pass over the logits and the uint8 labels each way (csrc/loss_ops.cu); no one-hot / probability volumes
-                dice_score, seg_ce = native_ops.seg_loss(seg_logits, seg.contiguous())
-                seg_dice = 1 - dice_score
-            else:
-                seg_ohe = F.one_hot(seg[:, 0], cf.num_seg_classes).movedim(-1, 1).float()  # on-device one-hot (reference: numpy, retina_unet.py:395)
-                seg_dice = 1 - batch_dice(F.softmax(seg_logits, dim=1), seg_ohe)
-                seg_ce = F.cross_entropy(seg_logits, seg[:, 0])
+            seg_dice, seg_ce = seg_loss_terms(seg_logits, seg, cf)
             loss = loss + (seg_dice + seg_ce) / 2
 
         detections = self._detect(class_logits, pred_deltas)
@@ -419,10 +318,13 @@ class net(nn.Module):
             # "mean pix. pr." of the logger string, reduced on the device (np.mean over the 4 M-voxel label map costs ms of host time per step)
             vals = torch.cat((vals, (seg_pred.sum(dtype=torch.float64) / seg_pred.numel()).to(vals.dtype).reshape(1)))
             to_host = [detections, vals, seg_pred]
-        host = self._to_host(to_host)
+        show = kwargs.get('monitor_anchors', True)
+        n_host = len(to_host)
+        host = self._to_host(to_host + ([t for pair in monitor for t in pair] if show else []))
         results_dict = get_results(cf, img.shape, detections, seg_logits, box_results_list, host=(host[0], host[2] if self.has_seg_head else None))
-        if kwargs.get('monitor_anchors', True):
-            self._append_anchor_boxes(results_dict['boxes'], monitor, img.shape[2:])
+        if show:
+            # positive / sampled-negative anchors for the monitoring plots (retina_unet.py:420-439)
+            append_anchor_boxes(self.np_anchors, host[n_host::2], host[n_host + 1::2], img.shape[2:], cf.dim, results_dict['boxes'])
         results_dict['torch_loss'] = loss
         vals = host[1].tolist()
         results_dict['monitor_values'] = {'loss': vals[0], 'class_loss': vals[1]}
@@ -432,20 +334,6 @@ class net(nn.Module):
         else:
             results_dict['logger_string'] = "loss: {0:.2f}, class: {1:.2f}, bbox: {2:.2f}".format(vals[0], vals[1], vals[2])
         return results_dict
-
-    def _append_anchor_boxes(self, boxes_list, monitor, spatial):
-        """positive / sampled-negative anchors for the monitoring plots (retina_unet.py:420-439)"""
-        hi = np.array([spatial[0], spatial[1], spatial[0], spatial[1]] + ([spatial[2], spatial[2]] if self.cf.dim == 3 else []))
-        for b, (match, neg_ix) in enumerate(monitor):
-            m = match.cpu().numpy()
-            pos = self.np_anchors[m > 0]
-            neg_all = np.where(m == -1)[0]
-            nix = neg_ix.cpu().numpy()
-            neg = self.np_anchors[neg_all[nix[nix >= 0]]] if neg_all.size else np.zeros((0, hi.size))
-            for p in np.clip(pos, 0, hi):
-                boxes_list[b].append({'box_coords': p, 'box_type': 'pos_anchor'})
-            for n in np.clip(neg, 0, hi):
-                boxes_list[b].append({'box_coords': n, 'box_type': 'neg_anchor'})
 
     def test_forward(self, batch, **kwargs):
         img = self._to_device(batch['data'])
