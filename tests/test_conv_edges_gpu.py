@@ -15,7 +15,13 @@ bar and those shapes cannot see:
     csrc/conv3d_stem.cu, each row names the plan it selects, and module-level assertions check that the rows reach every kernel
     instantiation, staging variant, scalar / 64-bit access path and persistent-loop regime (several tiles or line groups per CTA);
   * mdt_conv3d_backward with every combination of dx, y_relu and dy_masked_out, and a sweep asserting that a pass the dispatch selects runs;
-  * the fp32-path conv calls of one full-resolution retina_unet train step, each at its real shape against fp64.
+  * every conv call of one full-resolution retina_unet train step (3D, batch 2, 128^3: the bench configuration), listed in FULLRES_CALLS and
+    pinned to the step's own calls: the fp32-kernel calls at their real shapes against fp64, the tensor-core calls at their real shapes and
+    both precisions through the entry points the step uses (pre-split input, epilogue-emitted split planes, the fused backward fed from a
+    producer's epilogue), with a max-norm bound against fp64 that the per-element metric cannot replace at this size (a dropped CTA of the
+    chain-limited weight-gradient grid is near tau per element);
+  * the step itself, with every conv call checked against a reference built from that call's own operands, and the split planes a call
+    receives, finds cached or emits checked byte for byte against mdt_conv3d_split of their tensor.
 Inf is not covered: on the tensor cores an infinite operand becomes NaN by construction (its lo plane is inf - inf)."""
 import os
 import sys
@@ -25,7 +31,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from _guarded import _run_guarded
+from _guarded import OFFSETS, _run_guarded
 from medicaldetectiontoolkit_b200 import _lib as L
 from medicaldetectiontoolkit_b200 import conv as C
 
@@ -35,13 +41,14 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CL3 = torch.channels_last_3d
 
 # Bounds on e (see _err): 4x the worst value measured over the cases of this file on an H100 80GB HBM3 (power limit 400 W; later cases at
-# 700 W, noted below; tc-p0 keeps 2.8x the worst of a later case; the
+# 700 W, noted below; tc-p0 keeps 2.8x the worst of a later case and 1.5x the worst over the full-resolution calls, tc-p1 2.8x; the
 # kernels are deterministic, so the seeded cases give the same e on every run), within the caps 1e-4 (tensor cores against the emulated
 # operands) and 1e-5 (fp32 FMA kernels against fp64).  The module prints the worst e it saw when pytest runs with -s.
 TAU = {
     "tc-p0": 2.8e-5,   # split-bf16 x3 vs conv(xh,wh) + conv(xh,wl) + conv(xl,wh); measured worst 1.0e-5 (the tensor-core row of the fused
-                       # backward argument matrix, H100 80GB HBM3 at 700 W; 6.9e-6 over the other cases)
-    "tc-p1": 6.6e-7,   # single-pass bf16 vs conv(bf16(x), bf16(w)); measured worst 1.64e-7
+                       # backward argument matrix, H100 80GB HBM3 at 700 W; 6.9e-6 over the other cases); 1.81e-5 over the tensor-core calls of
+                       # the full-resolution train step (§12 - §14: weight gradients of up to 4.2 M products, H100 80GB HBM3, power limit 700 W)
+    "tc-p1": 6.6e-7,   # single-pass bf16 vs conv(bf16(x), bf16(w)); measured worst 1.64e-7; 2.32e-7 over the full-resolution calls (same card)
     "fp32": 1.8e-6,    # SIMT, stem and pointwise kernels, bias gradients vs fp64; measured worst 4.26e-7
     # pointwise weight gradients of the full-resolution layers: ~5,300 voxels (2 x 128^3 over 396 CTAs and 2 voxel groups) per fp32 accumulator
     # before the partials are added; measured worst 9.63e-8 (H100 80GB HBM3, power limit 700 W)
@@ -90,41 +97,43 @@ def _variants(g, algo):
     return "".join(str(lib.mdt_conv3d_variant(g.desc(algo=algo), ps)) for ps in range(3))
 
 
-def _fprop(g, algo, prec, x, w, b, res, relu=0):
+def _fprop(g, algo, prec, x, w, b, res, relu=0, offsets=OFFSETS):
     lib, d = L.load(), g.desc(relu, prec, algo)
     nws = lib.mdt_conv3d_workspace_bytes(d, 0)
     out = _run_guarded(lambda o, ws: lib.mdt_conv3d_fprop(d, L.ptr(x), L.ptr(w), L.ptr(b), L.ptr(res), o[0], ws, nws, L.stream_ptr()),
-                       [g.nbytes(g.yshape)], nws)
+                       [g.nbytes(g.yshape)], nws, offsets=offsets)
     return _ndhwc(out[0], g.n, g.cout, g.osp)
 
 
-def _dgrad(g, algo, prec, dy, w):
+def _dgrad(g, algo, prec, dy, w, offsets=OFFSETS):
     lib, d = L.load(), g.desc(0, prec, algo)
     nws = lib.mdt_conv3d_workspace_bytes(d, 1)
-    out = _run_guarded(lambda o, ws: lib.mdt_conv3d_dgrad(d, L.ptr(dy), L.ptr(w), o[0], ws, nws, L.stream_ptr()), [g.nbytes(g.xshape)], nws)
+    out = _run_guarded(lambda o, ws: lib.mdt_conv3d_dgrad(d, L.ptr(dy), L.ptr(w), o[0], ws, nws, L.stream_ptr()), [g.nbytes(g.xshape)], nws,
+                       offsets=offsets)
     return _ndhwc(out[0], g.n, g.cin, g.sp)
 
 
-def _wgrad(g, algo, prec, x, dy):
+def _wgrad(g, algo, prec, x, dy, offsets=OFFSETS):
     lib, d = L.load(), g.desc(0, prec, algo)
     nws = lib.mdt_conv3d_workspace_bytes(d, 2)
     out = _run_guarded(lambda o, ws: lib.mdt_conv3d_wgrad(d, L.ptr(x), L.ptr(dy), o[0], o[1], ws, nws, L.stream_ptr()),
-                       [g.nbytes(g.wshape), g.cout * 4], nws)
+                       [g.nbytes(g.wshape), g.cout * 4], nws, offsets=offsets)
     dw, db = _f32(out[0], *g.wshape), _f32(out[1], g.cout)
     assert bool(torch.isfinite(dw).all() and torch.isfinite(db).all())
     return dw, db
 
 
-def _split(g, prec, x):
+def _split(g, prec, x, offsets=OFFSETS):
     """canonical split form of the input x of g (mdt_conv3d_split), written into a guarded poisoned buffer"""
     lib, d = L.load(), g.desc(0, prec, 2)
-    return _run_guarded(lambda o, ws: lib.mdt_conv3d_split(d, L.ptr(x), o[0], L.stream_ptr()), [lib.mdt_conv3d_split_bytes(d)], None)[0]
+    return _run_guarded(lambda o, ws: lib.mdt_conv3d_split(d, L.ptr(x), o[0], L.stream_ptr()), [lib.mdt_conv3d_split_bytes(d)], None,
+                        offsets=offsets)[0]
 
 
-def _check_out_split(g, prec, y, ys):
+def _check_out_split(g, prec, y, ys, offsets=OFFSETS):
     """ys (emitted by a conv epilogue) must be byte-identical to mdt_conv3d_split of its fp32 result y, with byte-zero padding channels"""
     gy = Geo(g.n, g.cout, 16, 1, 1, 0, g.osp)
-    want = _split(gy, prec, y.contiguous(memory_format=CL3))
+    want = _split(gy, prec, y.contiguous(memory_format=CL3), offsets)
     assert ys.numel() == want.numel() and torch.equal(ys, want), int((ys != want).sum())
     planes, kg = 2 - prec, (g.cout + 15) // 16 * 16
     lines = g.n * g.osp[0] * g.osp[1]
@@ -132,16 +141,16 @@ def _check_out_split(g, prec, y, ys):
     assert bool((data[..., g.cout:] == 0).all()), "padding channels of the split planes are not zero"
 
 
-def _fprop_presplit(g, prec, xs, w, b, res, relu, out_split):
+def _fprop_presplit(g, prec, xs, w, b, res, relu, out_split, offsets=OFFSETS):
     lib, d = L.load(), g.desc(relu, prec, 2)
     nws = lib.mdt_conv3d_workspace_bytes(d, 0)
     if out_split:
         out = _run_guarded(lambda o, ws: lib.mdt_conv3d_fprop_presplit_out(d, L.ptr(xs), L.ptr(w), L.ptr(b), L.ptr(res), o[0], o[1], ws, nws,
                                                                            L.stream_ptr()),
-                           [g.nbytes(g.yshape), lib.mdt_conv3d_out_split_bytes(d)], nws)
+                           [g.nbytes(g.yshape), lib.mdt_conv3d_out_split_bytes(d)], nws, offsets=offsets)
         return _ndhwc(out[0], g.n, g.cout, g.osp), out[1]
     out = _run_guarded(lambda o, ws: lib.mdt_conv3d_fprop_presplit(d, L.ptr(xs), L.ptr(w), L.ptr(b), L.ptr(res), o[0], ws, nws, L.stream_ptr()),
-                       [g.nbytes(g.yshape)], nws)
+                       [g.nbytes(g.yshape)], nws, offsets=offsets)
     return _ndhwc(out[0], g.n, g.cout, g.osp)
 
 
@@ -154,13 +163,13 @@ def _fprop_out(g, x, w, b, res, relu, prec=0):
     return _ndhwc(out[0], g.n, g.cout, g.osp), out[1]
 
 
-def _backward(g, prec, x, x_split, dy, y_relu, w, need_dx, want_masked, algo=0):
+def _backward(g, prec, x, x_split, dy, y_relu, w, need_dx, want_masked, algo=0, offsets=OFFSETS):
     """mdt_conv3d_backward -> (dx | None, dw, db, dy_masked | None)"""
     lib, d = L.load(), g.desc(0, prec, algo)
     nws = lib.mdt_conv3d_backward_workspace_bytes(d, int(need_dx))
     outs = [g.nbytes(g.xshape) if need_dx else None, g.nbytes(g.wshape), g.cout * 4, g.nbytes(g.yshape) if want_masked else None]
     out = _run_guarded(lambda o, ws: lib.mdt_conv3d_backward(d, L.ptr(x), L.ptr(x_split), L.ptr(dy), L.ptr(y_relu), L.ptr(w), o[0], o[1], o[2], o[3],
-                                                             ws, nws, L.stream_ptr()), outs, nws)
+                                                             ws, nws, L.stream_ptr()), outs, nws, offsets=offsets)
     dx = _ndhwc(out[0], g.n, g.cin, g.sp) if need_dx else None
     gm = _ndhwc(out[3], g.n, g.cout, g.osp) if want_masked else None
     dw, db = _f32(out[1], *g.wshape), _f32(out[2], g.cout)
@@ -202,6 +211,13 @@ def _check(tag, y, ref, mag):
     e = _err(y, ref, mag)
     _WORST[tag] = max(_WORST.get(tag, 0.0), e)
     assert e <= TAU[tag], (tag, e, TAU[tag])
+    return e
+
+
+def _check_fullres(tag, y, ref, mag):
+    """_check for the calls of the full-resolution train step, whose worst e is also reported on its own"""
+    key = tag + " (full resolution)"
+    _WORST[key] = max(_WORST.get(key, 0.0), _check(tag, y, ref, mag))
 
 
 def _operands(g, seed):
@@ -899,10 +915,10 @@ def test_dispatch_accepts_what_it_selects():
     assert not bad, bad
 
 
-# ------------------------------------------------------------------------------------------------ §10 full resolution: the fp32-path convs of a train step
-# (pass, x shape, w shape, stride, kernel) of every conv call on the fp32 kernels (stem, SIMT, pointwise) in one retina_unet train step at the
-# bench configuration (3D, batch 2, 128^3), as conv.EVENT_LOG tags them: pass 0 fprop, 1 dgrad, 2 wgrad, 3 fused backward; kernel 1 = SIMT /
-# stem, 4 = pointwise
+# ------------------------------------------------------------------------------------------------ §10 full resolution: every conv call of a train step
+# (pass, x shape, w shape, stride, kernel) of every conv call in one retina_unet train step at the bench configuration (3D, batch 2, 128^3),
+# as conv.EVENT_LOG tags them: pass 0 fprop, 1 dgrad, 2 wgrad, 3 fused backward; kernel 1 = SIMT / stem, 2 = tensor cores, 4 = pointwise.
+# Every conv of the model pads by k // 2 (test_full_resolution_call_list asserts it), so the table leaves the padding out.
 FULLRES_CALLS = [
     (0, (2, 1, 128, 128, 128), (18, 1, 3, 3, 3), (1, 1, 1), 1),
     (0, (2, 18, 32, 32, 128), (18, 18, 1, 1, 1), (1, 1, 1), 4),
@@ -938,25 +954,113 @@ FULLRES_CALLS = [
     (3, (2, 36, 128, 128, 128), (2, 36, 1, 1, 1), (1, 1, 1), 4),
     (3, (2, 72, 32, 32, 128), (18, 72, 1, 1, 1), (1, 1, 1), 4),
     (3, (2, 72, 32, 32, 128), (36, 72, 1, 1, 1), (1, 1, 1), 4),
+    # tensor cores: 3x3x3 convs of the encoder, the FPN and the heads, the 7x7x7 stride-(2,2,1) C1, 1x1x1 convs with cin * cout > 2592; the
+    # two with cout > 256 run unfused dgrad and wgrad (passes 1 and 2)
+    (0, (2, 18, 32, 32, 128), (18, 18, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 18, 128, 128, 128), (18, 18, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 18, 128, 128, 128), (18, 18, 7, 7, 7), (2, 2, 1), 2),
+    (0, (2, 36, 4, 4, 16), (36, 36, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 36, 4, 4, 16), (64, 36, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 36, 8, 8, 32), (36, 36, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 36, 8, 8, 32), (64, 36, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 36, 16, 16, 64), (36, 36, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 36, 16, 16, 64), (64, 36, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 36, 16, 16, 64), (144, 36, 1, 1, 1), (1, 1, 1), 2),
+    (0, (2, 36, 32, 32, 128), (36, 36, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 36, 32, 32, 128), (64, 36, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 36, 128, 128, 128), (36, 36, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 64, 4, 4, 16), (27, 64, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 64, 4, 4, 16), (54, 64, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 64, 4, 4, 16), (64, 64, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 64, 8, 8, 32), (27, 64, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 64, 8, 8, 32), (54, 64, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 64, 8, 8, 32), (64, 64, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 64, 16, 16, 64), (27, 64, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 64, 16, 16, 64), (54, 64, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 64, 16, 16, 64), (64, 64, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 64, 32, 32, 128), (27, 64, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 64, 32, 32, 128), (54, 64, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 64, 32, 32, 128), (64, 64, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 72, 8, 8, 32), (72, 72, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 72, 8, 8, 32), (288, 72, 1, 1, 1), (1, 1, 1), 2),
+    (0, (2, 144, 4, 4, 16), (144, 144, 3, 3, 3), (1, 1, 1), 2),
+    (0, (2, 144, 4, 4, 16), (576, 144, 1, 1, 1), (1, 1, 1), 2),
+    (0, (2, 144, 16, 16, 64), (36, 144, 1, 1, 1), (1, 1, 1), 2),
+    (0, (2, 288, 8, 8, 32), (36, 288, 1, 1, 1), (1, 1, 1), 2),
+    (0, (2, 288, 8, 8, 32), (72, 288, 1, 1, 1), (1, 1, 1), 2),
+    (0, (2, 576, 4, 4, 16), (36, 576, 1, 1, 1), (1, 1, 1), 2),
+    (0, (2, 576, 4, 4, 16), (144, 576, 1, 1, 1), (1, 1, 1), 2),
+    (1, (2, 72, 8, 8, 32), (288, 72, 1, 1, 1), (1, 1, 1), 2),
+    (1, (2, 144, 4, 4, 16), (576, 144, 1, 1, 1), (1, 1, 1), 2),
+    (2, (2, 72, 8, 8, 32), (288, 72, 1, 1, 1), (1, 1, 1), 2),
+    (2, (2, 144, 4, 4, 16), (576, 144, 1, 1, 1), (1, 1, 1), 2),
+    (3, (2, 18, 32, 32, 128), (18, 18, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 18, 128, 128, 128), (18, 18, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 18, 128, 128, 128), (18, 18, 7, 7, 7), (2, 2, 1), 2),
+    (3, (2, 36, 4, 4, 16), (36, 36, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 36, 4, 4, 16), (64, 36, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 36, 8, 8, 32), (36, 36, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 36, 8, 8, 32), (64, 36, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 36, 16, 16, 64), (36, 36, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 36, 16, 16, 64), (64, 36, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 36, 16, 16, 64), (144, 36, 1, 1, 1), (1, 1, 1), 2),
+    (3, (2, 36, 32, 32, 128), (36, 36, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 36, 32, 32, 128), (64, 36, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 36, 128, 128, 128), (36, 36, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 64, 4, 4, 16), (27, 64, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 64, 4, 4, 16), (54, 64, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 64, 4, 4, 16), (64, 64, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 64, 8, 8, 32), (27, 64, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 64, 8, 8, 32), (54, 64, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 64, 8, 8, 32), (64, 64, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 64, 16, 16, 64), (27, 64, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 64, 16, 16, 64), (54, 64, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 64, 16, 16, 64), (64, 64, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 64, 32, 32, 128), (27, 64, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 64, 32, 32, 128), (54, 64, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 64, 32, 32, 128), (64, 64, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 72, 8, 8, 32), (72, 72, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 144, 4, 4, 16), (144, 144, 3, 3, 3), (1, 1, 1), 2),
+    (3, (2, 144, 16, 16, 64), (36, 144, 1, 1, 1), (1, 1, 1), 2),
+    (3, (2, 288, 8, 8, 32), (36, 288, 1, 1, 1), (1, 1, 1), 2),
+    (3, (2, 288, 8, 8, 32), (72, 288, 1, 1, 1), (1, 1, 1), 2),
+    (3, (2, 576, 4, 4, 16), (36, 576, 1, 1, 1), (1, 1, 1), 2),
+    (3, (2, 576, 4, 4, 16), (144, 576, 1, 1, 1), (1, 1, 1), 2),
 ]
 
 
-def test_full_resolution_fp32_call_list():
-    """FULLRES_CALLS is exactly the set of stem and pointwise conv calls of one train step: a new layer shape cannot go untested"""
+FULLRES_FP32 = [c for c in FULLRES_CALLS if c[4] != 2]
+FULLRES_TC = [c for c in FULLRES_CALLS if c[4] == 2]
+FULLRES_MAXNORM = 3e-5   # precision 0 against plain fp64 at 2 x 128^3, relative to max|ref|: what the wgrad accumulator chain limit guarantees
+
+
+def _bench_train_step():
+    """one retina_unet train step (forward and backward) at the bench configuration: 3D, batch 2, 128^3, seeded"""
     from medicaldetectiontoolkit_b200 import retina_unet
     from medicaldetectiontoolkit_b200.configs import make_cf, synthetic_batch
     cf = make_cf('retina_unet', 3, (128, 128, 128), batch_size=2)
     torch.manual_seed(0)
     net = retina_unet.net(cf, None).to(DEV)
-    C.EVENT_LOG = []
-    try:
-        res = net.train_forward(synthetic_batch(cf, 2, seed=0), monitor_anchors=False)
-        res['torch_loss'].backward()
-        torch.cuda.synchronize()
-        got = sorted({tag for _, _, tag in C.EVENT_LOG if tag is not None and tag[4] in (1, 4)})
-    finally:
-        C.EVENT_LOG = None
-    assert got == sorted(FULLRES_CALLS), got
+    res = net.train_forward(synthetic_batch(cf, 2, seed=0), monitor_anchors=False)
+    res['torch_loss'].backward()
+    torch.cuda.synchronize()
+    assert np.isfinite(float(res['torch_loss'].detach()))
+    return net
+
+
+def test_full_resolution_call_list(monkeypatch):
+    """FULLRES_CALLS is exactly the set of conv calls of one train step at either precision, and every call runs on kernel 1, 2 or 4: a new
+    layer shape or a changed kernel choice cannot go untested.  Every conv module pads by k // 2, as the per-call tests assume."""
+    for prec in (0, 1):
+        monkeypatch.setattr(C, "DEFAULT_PRECISION", prec)
+        monkeypatch.setattr(C, "EVENT_LOG", [])
+        net = _bench_train_step()
+        got = sorted({tag for _, _, tag in C.EVENT_LOG})
+        convs = [m for m in net.modules() if isinstance(m, C.Conv3d)]
+        assert convs and all(m.padding == tuple(k // 2 for k in m.kernel_size) for m in convs)
+        assert {tag[4] for tag in got} <= {1, 2, 4}, got
+        assert got == sorted(FULLRES_CALLS), (prec, got)
+        del net
 
 
 def _fullres_operands(g, seed):
@@ -969,13 +1073,22 @@ def _fullres_operands(g, seed):
     return x, w, b, dy
 
 
-@pytest.mark.parametrize("call", FULLRES_CALLS, ids=["p%d_%s_%s" % (c[0], "x".join(map(str, c[1])), "x".join(map(str, c[2]))) for c in FULLRES_CALLS])
-def test_full_resolution_fp32_layers_vs_fp64(call):
-    """each call of FULLRES_CALLS at its real shape against fp64 (einsum for 1x1x1, F.conv3d and grad.conv3d_weight for the stem).  The
-    pointwise weight gradient sums thousands of voxels into one fp32 accumulator per CTA: it has a bound of its own, fp32-fullres."""
+def _fullres_geo(call):
     ps, xs, ws, st, which = call
     k = tuple(ws[2:])
-    g = Geo(xs[0], xs[1], ws[0], k, st, tuple(kk // 2 for kk in k), xs[2:])
+    return Geo(xs[0], xs[1], ws[0], k, st, tuple(kk // 2 for kk in k), xs[2:])
+
+
+def _call_id(c):
+    return "p%d_%s_%s" % (c[0], "x".join(map(str, c[1])), "x".join(map(str, c[2])))
+
+
+@pytest.mark.parametrize("call", FULLRES_FP32, ids=[_call_id(c) for c in FULLRES_FP32])
+def test_full_resolution_fp32_layers_vs_fp64(call):
+    """each fp32-kernel call of FULLRES_CALLS at its real shape against fp64 (einsum for 1x1x1, F.conv3d and grad.conv3d_weight for the stem).
+    The pointwise weight gradient sums thousands of voxels into one fp32 accumulator per CTA: it has a bound of its own, fp32-fullres."""
+    ps, xs, ws, st, which = call
+    g = _fullres_geo(call)
     x, w, b, dy = _fullres_operands(g, sum(xs) + sum(ws) + ps)
     fwd, dgr, wgr = _pw_ops() if which == 4 else _ops(g)
     algo = which
@@ -1024,3 +1137,314 @@ def test_fp32_metric_catches_a_planted_error(kind, ps):
         b64[5, 0, tuple(kk // 2 for kk in g.k)[0], g.k[1] // 2, 0] = 0.0
     e = _err(got, op(a64, b64), mag)
     assert e >= 3 * tau, (e, tau)
+
+
+# ------------------------------------------------------------------------------------------------ §12 full resolution: the tensor-core convs of a train step
+def _no_experiment_knobs():
+    """the restated plans and the rows' kernel choices assume the default settings of the tensor-core kernels"""
+    knobs = sorted(k for k in os.environ if k.startswith(("MDT_TC_", "MDT_WG_")))
+    assert not knobs, knobs
+
+
+def _tc_check(prec, got, emul, mag, ref64):
+    """the per-element bound against the emulated operands and, at precision 0, the full-resolution max-norm bound against plain fp64"""
+    _check_fullres("tc-p%d" % prec, got, emul, mag)
+    if prec == 0:
+        e = _maxnorm(got, ref64)
+        _WORST["maxnorm-fullres"] = max(_WORST.get("maxnorm-fullres", 0.0), e)
+        assert e <= FULLRES_MAXNORM, (e, FULLRES_MAXNORM)
+
+
+def _bias_check(prec, db, dy64):
+    _check("fp32", db, dy64.sum((0, 2, 3, 4)), dy64.abs().sum((0, 2, 3, 4)))
+    if prec == 0:
+        assert _maxnorm(db, dy64.sum((0, 2, 3, 4))) <= FULLRES_MAXNORM
+
+
+@pytest.mark.parametrize("call", FULLRES_TC, ids=[_call_id(c) for c in FULLRES_TC])
+def test_full_resolution_tc_layers(call):
+    """each tensor-core call of FULLRES_CALLS at its real shape and at both precisions, through the entry points the train step uses.
+    fprop (pass 0): mdt_conv3d_fprop with bias and residual; mdt_conv3d_fprop_presplit on mdt_conv3d_split(x) bit-identical to it; the
+    ReLU epilogue that also emits the split planes of its result.  Fused backward (pass 3): x is the ReLU output of a producer conv whose
+    epilogue emitted x's split planes, the mask comes from our own forward, dx and dy_masked_out are requested; the result must not depend
+    on where the split of x comes from, and the standalone dgrad and wgrad of the masked dy share its references.  dgrad / wgrad (passes 1
+    and 2): the layers with cout > 256, where the fused backward does not apply.  One buffer offset (the offset matrix is a small-shape
+    property, covered by §2), both workspace fills."""
+    _no_experiment_knobs()
+    ps, xs_, ws_, st, _ = call
+    g = _fullres_geo(call)
+    lib = L.load()
+    off = (0,)
+    x, w, b, dy = _fullres_operands(g, sum(xs_) + sum(ws_) + ps)
+    fwd, dgr, wgr = _ops(g)
+    w64 = w.double()
+    if ps == 0:
+        assert lib.mdt_conv3d_variant(g.desc(), 0) == 2
+        torch.manual_seed(sum(xs_) + 1)
+        res = torch.randn(g.yshape, device=DEV).contiguous(memory_format=CL3)
+        b64, r64, x64 = b.double().view(1, -1, 1, 1, 1), res.double(), x.double()
+        extra = b64 + r64
+        y64, y_mag = fwd(x64, w64) + extra, fwd(x64.abs(), w64.abs()) + b64.abs() + r64.abs()
+        del x64
+        for prec in (0, 1):
+            y = _fprop(g, 2, prec, x, w, b, res, offsets=off)
+            _tc_check(prec, y, _emul(fwd, x, w, prec) + extra, y_mag, y64)
+            xs = _split(g, prec, x, off)
+            assert torch.equal(_fprop_presplit(g, prec, xs, w, b, res, 0, False, off), y)
+            yr, ys = _fprop_presplit(g, prec, xs, w, b, res, 1, True, off)
+            assert torch.equal(yr, torch.relu(y))
+            _check_out_split(g, prec, yr, ys, off)
+        return
+    if ps in (1, 2):
+        assert lib.mdt_conv3d_variant(g.desc(), ps) == 2 and lib.mdt_conv3d_backward_fused(g.desc(), 1) == 0 and g.cout > 256
+        dy64 = dy.double()
+        if ps == 1:
+            ref, mag = dgr(dy64, w64), dgr(dy64.abs(), w64.abs())
+        else:
+            x64 = x.double()
+            ref, mag = wgr(x64, dy64), wgr(x64.abs(), dy64.abs())
+        for prec in (0, 1):
+            if ps == 1:
+                _tc_check(prec, _dgrad(g, 2, prec, dy, w, off), _emul(dgr, dy, w, prec), mag, ref)
+            else:
+                dw, db = _wgrad(g, 2, prec, x, dy, off)
+                _tc_check(prec, dw, _emul(wgr, x, dy, prec), mag, ref)
+                _bias_check(prec, db, dy64)
+        return
+    assert ps == 3 and lib.mdt_conv3d_backward_fused(g.desc(), 1) == 1
+    gp = Geo(g.n, 16, g.cin, 1, 1, 0, g.sp)
+    x0, wp, bp, _ = _fullres_operands(gp, 5)
+    for prec in (0, 1):
+        x, x_split_epi = _fprop_presplit(gp, prec, _split(gp, prec, x0, off), wp, bp, None, 1, True, off)
+        x = x.contiguous(memory_format=CL3)
+        y = C.conv3d_forward(x, w, b, g.s, g.p, relu=True, precision=prec)
+        dym = torch.ops.aten.threshold_backward(dy, y, 0.0)
+        dx, dw, db, gm = _backward(g, prec, x, x_split_epi, dy, y, w, True, True, offsets=off)
+        assert torch.equal(gm, dym)
+        again = _backward(g, prec, x, None, dy, y, w, True, True, offsets=off)   # the backward splits x itself
+        assert all(torch.equal(a, b_) for a, b_ in zip((dx, dw, db, gm), again))
+        del y, gm, again
+        x64, dym64 = x.double(), dym.double()
+        dx_ref, dx_mag = dgr(dym64, w64), dgr(dym64.abs(), w64.abs())
+        dx_emul = _emul(dgr, dym, w, prec)
+        _tc_check(prec, dx, dx_emul, dx_mag, dx_ref)
+        _tc_check(prec, _dgrad(g, 2, prec, dym, w, off), dx_emul, dx_mag, dx_ref)
+        del dx, dx_ref, dx_mag, dx_emul
+        dw_ref, dw_mag, dw_emul = wgr(x64, dym64), wgr(x64.abs(), dym64.abs()), _emul(wgr, x, dym, prec)
+        _tc_check(prec, dw, dw_emul, dw_mag, dw_ref)
+        _bias_check(prec, db, dym64)
+        dw2, db2 = _wgrad(g, 2, prec, x, dym, off)
+        _tc_check(prec, dw2, dw_emul, dw_mag, dw_ref)
+        _bias_check(prec, db2, dym64)
+        del x, x64, dym, dym64, x_split_epi
+
+
+# ------------------------------------------------------------------------------------------------ §13 sensitivity at full resolution
+def _kpad_smem(c):
+    """conv_tc_kpad_smem (csrc/conv3d_tc.cu:353): channels staged in shared memory"""
+    return 16 if c <= 16 else 32 if c <= 32 else _cdiv(c, 64) * 64
+
+
+def _wg_plan(g, sms):
+    """split-K plan of the tensor-core weight gradient at the default settings: make_wg_plan and wg_splits (csrc/conv3d_tc_wgrad.cu:213-274).
+    A CTA of split s takes the work units (output lines when W <= 128) s, s + splits, ...; the chain limit kMaxChain = 512 MMAs per accumulator
+    caps the units per CTA, and a wave of 2 CTAs per SM sets the split count from below."""
+    chunkx = min(_kpad_smem(g.cin), 64)
+    co_p = _kpad_smem(g.cout)
+    mtrick = 2 * co_p <= 128
+    mtiles = 1 if mtrick else _cdiv(co_p, 128)
+    ow = g.osp[2]
+    seg = min(ow, 128)
+    segs, ksteps = _cdiv(ow, seg), _cdiv(seg, 16)
+    groups = g.k[0] * g.k[1] * (_kpad_smem(g.cin) // chunkx)
+    units = g.n * g.osp[0] * g.osp[1] * segs
+    chain = _cdiv(units, max(512 // (ksteps * (2 if mtrick else 3)), 1))
+    wave = sms * 2 // (groups * mtiles)
+    splits = min(max(chain, wave, 1), units)
+    return dict(units=units, segs=segs, splits=splits, chain_limited=chain > wave,
+                partial_bytes=splits * groups * mtiles * 128 * _cdiv(g.k[2] * chunkx, 16) * 16 * 4)
+
+
+def _wg_workspace_bytes(g, prec, sms):
+    """mdt_conv3d_workspace_bytes of the tensor-core weight gradient (conv_tc_wgrad_workspace_bytes, :278-286, and bias_grad_blocks,
+    csrc/conv3d_simt.cu:290-295): the split planes of dy and x, the partial buffer of the split-K plan, the bias-gradient partials"""
+    al = lambda v: _cdiv(v, 1024) * 1024
+    rows_y, rows_x = g.n * int(np.prod(g.osp)), g.n * int(np.prod(g.sp))
+    bias_blocks = min(_cdiv(rows_y, 32 if g.cout > 256 else 1024 if rows_y >= 262144 else 128), sms * 8)
+    return (al((2 - prec) * rows_y * _cdiv(g.cout, 16) * 16 * 2) + al((2 - prec) * rows_x * _cdiv(g.cin, 16) * 16 * 2) +
+            al(_wg_plan(g, sms)["partial_bytes"]) + al(bias_blocks * g.cout * 4) + 2048 + 256)
+
+
+def test_full_resolution_metrics_catch_a_planted_error():
+    """P0_conv2 (36 -> 36, k3) at 2 x 128^3.  Its weight gradient runs in the chain-limited regime (1024 splits of 32 lines each): one CTA of
+    that split-K grid dropped is about 1e-5 of mag, near tau, but about 1e-2 of max|ref|, so the max-norm bound is what sees it.  With the
+    lines of the last split zeroed in the reference's dy, the kernel's result fails that bound by >= 3x; with one input voxel (the last row of
+    the last tile of the last line of the last sample) zeroed in the reference operand, fprop and dgrad fail the per-element bound by >= 3
+    tau.  Unplanted, all three pass."""
+    _no_experiment_knobs()
+    g = Geo(2, 36, 36, 3, 1, 1, (128, 128, 128))
+    assert (3, (2, 36, 128, 128, 128), (36, 36, 3, 3, 3), (1, 1, 1), 2) in FULLRES_CALLS   # the fused backward runs the same wgrad plan
+    lib, sms = L.load(), _sms()
+    plan = _wg_plan(g, sms)
+    assert lib.mdt_conv3d_workspace_bytes(g.desc(0, 0, 2), 2) == _wg_workspace_bytes(g, 0, sms)
+    assert plan["chain_limited"] and plan["segs"] == 1 and plan["units"] // plan["splits"] == 32, plan
+    x, w, _, dy = _fullres_operands(g, 61)
+    fwd, dgr, wgr = _ops(g)
+    tau = TAU["tc-p0"]
+    # weight gradient: the max-norm against plain fp64
+    dw, _ = _wgrad(g, 2, 0, x, dy, offsets=(0,))
+    x64 = x.double()
+    assert _maxnorm(dw, wgr(x64, dy.double())) <= FULLRES_MAXNORM
+    u = torch.arange(plan["splits"] - 1, plan["units"], plan["splits"], device=DEV)   # unit = (n * OD + od) * OH + oh
+    oh, od, n = u % g.osp[1], (u // g.osp[1]) % g.osp[0], u // (g.osp[1] * g.osp[0])
+    dy2 = dy.double()
+    dy2[n, :, od, oh, :] = 0.0
+    e = _maxnorm(dw, wgr(x64, dy2))
+    assert e >= 3 * FULLRES_MAXNORM, e
+    del dy2, x64
+    # fprop and dgrad: the per-element metric against the emulated operands
+    for op, a, b_, got in ((fwd, x, w, _fprop(g, 2, 0, x, w, None, None, offsets=(0,))), (dgr, dy, w, _dgrad(g, 2, 0, dy, w, offsets=(0,)))):
+        mag = op(a.double().abs(), b_.double().abs())
+        assert _err(got, _emul(op, a, b_, 0), mag) <= tau
+        a2 = a.clone()
+        a2[1, :, 127, 127, 127] = 0.0
+        e = _err(got, _emul(op, a2, b_, 0), mag)
+        assert e >= 3 * tau, e
+
+
+# ------------------------------------------------------------------------------------------------ §14 one train step, every conv call shadow-checked
+def _split_bytes_used(t, prec):
+    """bytes of the split planes of activation t that carry data: the allocation rounds up to 1 KiB"""
+    return (2 - prec) * t.shape[0] * int(np.prod(t.shape[2:])) * _cdiv(t.shape[1], 16) * 16 * 2
+
+
+def _canonical_split(t, prec):
+    """mdt_conv3d_split(t) in a fresh buffer"""
+    n, c, d, h, w = t.shape
+    lib, desc = L.load(), Geo(n, c, 16, 1, 1, 0, (d, h, w)).desc(0, prec, 2)
+    out = torch.empty(lib.mdt_conv3d_split_bytes(desc), dtype=torch.uint8, device=t.device)
+    L.check(lib.mdt_conv3d_split(desc, L.ptr(t.contiguous(memory_format=CL3)), L.ptr(out), L.stream_ptr()))
+    return out
+
+
+def _assert_split_of(what, planes, t, prec):
+    k = _split_bytes_used(t, prec)
+    assert planes.numel() >= k and torch.equal(planes[:k], _canonical_split(t, prec)[:k]), what + " is not the split of its tensor"
+
+
+class _Shadow:
+    """Stands in for conv.conv3d_forward / conv3d_dgrad / conv3d_wgrad / conv3d_backward (which _Conv3dFn looks up as module globals): each
+    real call is checked against a reference computed from that call's own operands (x, w, bias, residual, dy and the ReLU mask it
+    received), with the kernel-level bound of the kernel it ran on; the split planes a call receives, finds cached on its input or emits
+    must be byte-equal to mdt_conv3d_split of their tensor.  tags counts the checked calls per conv.EVENT_LOG tag."""
+
+    def __init__(self):
+        self.real = {n: getattr(C, "conv3d_" + n) for n in ("forward", "dgrad", "wgrad", "backward")}
+        self.tags = {}
+
+    def install(self, monkeypatch):
+        for n in self.real:
+            monkeypatch.setattr(C, "conv3d_" + n, getattr(self, n))
+
+    @staticmethod
+    def _plan(x_shape, w_shape, stride, padding, precision, algo, ps):
+        prec = C.DEFAULT_PRECISION if precision is None else precision
+        algo = C.DEFAULT_ALGO if algo is None else algo
+        d = C._desc(tuple(x_shape), tuple(w_shape), tuple(stride), tuple(padding), False, prec, algo)
+        g = Geo(x_shape[0], x_shape[1], w_shape[0], tuple(w_shape[2:]), tuple(stride), tuple(padding), tuple(x_shape[2:]))
+        return prec, L.load().mdt_conv3d_algo(d, ps), g
+
+    def _count(self, ps, x_shape, w_shape, stride, which):
+        tag = (ps, tuple(x_shape), tuple(w_shape), tuple(stride), which)
+        self.tags[tag] = self.tags.get(tag, 0) + 1
+
+    @staticmethod
+    def _check(which, prec, got, op, a, b, extra=0.0, extra_mag=0.0, relu=False, fp32_tag="fp32"):
+        a64, b64 = a.double(), b.double()
+        ref = (_emul(op, a, b, prec) if which == 2 else op(a64, b64)) + extra
+        _check_fullres("tc-p%d" % prec if which == 2 else fp32_tag, got, torch.relu(ref) if relu else ref, op(a64.abs(), b64.abs()) + extra_mag)
+
+    def forward(self, x, weight, bias, stride, padding, relu=False, residual=None, precision=None, algo=None, want_split=False, emit_split=False):
+        prec, which, g = self._plan(x.shape, weight.shape, stride, padding, precision, algo, 0)
+        hit = getattr(x, "_mdt_split", None)
+        if which == 2 and hit is not None and hit[1] == x._version and hit[2] == prec:
+            _assert_split_of("the split cached on the input", hit[0], x, prec)
+        out = self.real["forward"](x, weight, bias, stride, padding, relu, residual, precision, algo, want_split, emit_split)
+        y, xs = out if want_split else (out, None)
+        if xs is not None:
+            _assert_split_of("the split the forward read", xs, x, prec)
+        emitted = getattr(y, "_mdt_split", None)
+        if emitted is not None:
+            _assert_split_of("the split planes emitted by the epilogue", emitted[0], y, emitted[2])
+        extra, extra_mag = 0.0, 0.0
+        if bias is not None:
+            extra, extra_mag = bias.double().view(1, -1, 1, 1, 1), bias.double().abs().view(1, -1, 1, 1, 1)
+        if residual is not None:
+            extra, extra_mag = extra + residual.double(), extra_mag + residual.double().abs()
+        self._check(which, prec, y, _ops(g)[0], x, weight, extra, extra_mag, relu)
+        self._count(0, x.shape, weight.shape, stride, which)
+        return out
+
+    def dgrad(self, dy, weight, x_shape, stride, padding, precision=None, algo=None):
+        prec, which, g = self._plan(x_shape, weight.shape, stride, padding, precision, algo, 1)
+        dx = self.real["dgrad"](dy, weight, x_shape, stride, padding, precision, algo)
+        self._check(which, prec, dx, _ops(g)[1], dy, weight)
+        self._count(1, x_shape, weight.shape, stride, which)
+        return dx
+
+    def _grads(self, which, prec, g, x, dym, weight, dx, dw, db):
+        _, dgr, wgr = _ops(g)
+        self._check(which, prec, dw, wgr, x, dym, fp32_tag="fp32-fullres" if which == 4 else "fp32")
+        if db is not None:
+            dym64 = dym.double()
+            _check_fullres("fp32", db, dym64.sum((0, 2, 3, 4)), dym64.abs().sum((0, 2, 3, 4)))
+        if dx is not None:
+            self._check(which, prec, dx, dgr, dym, weight)
+
+    def wgrad(self, x, dy, w_shape, stride, padding, want_bias, precision=None, algo=None):
+        prec, which, g = self._plan(x.shape, w_shape, stride, padding, precision, algo, 2)
+        dw, db = self.real["wgrad"](x, dy, w_shape, stride, padding, want_bias, precision, algo)
+        self._grads(which, prec, g, x, dy, None, None, dw, db)
+        self._count(2, x.shape, w_shape, stride, which)
+        return dw, db
+
+    def backward(self, x, gy, y_relu, weight, stride, padding, need_dx, want_bias, want_masked, precision=None, algo=None, x_split=None):
+        prec, which, g = self._plan(x.shape, weight.shape, stride, padding, precision, algo, 2)
+        if x_split is not None:
+            _assert_split_of("the x_split handed to the backward", x_split, x, prec)
+        out = self.real["backward"](x, gy, y_relu, weight, stride, padding, need_dx, want_bias, want_masked, precision, algo, x_split)
+        if out is None:   # the fused path does not apply: the caller runs dgrad and wgrad, which are checked on their own
+            return None
+        dx, dw, db, gm = out
+        dym = gy if y_relu is None else torch.ops.aten.threshold_backward(gy, y_relu, 0.0)
+        if want_masked:
+            assert torch.equal(gm, dym)
+        self._grads(which, prec, g, x, dym, weight, dx, dw, db)
+        self._count(3, x.shape, weight.shape, stride, which)
+        return out
+
+
+def test_train_step_every_conv_call_on_its_own_operands(monkeypatch):
+    """one retina_unet train step at the bench configuration (precision 0), every conv call checked by _Shadow.  Conditioned on the step's
+    own upstream values, no ReLU flip can move a reference, so every call gets the kernel-level bound rather than a model-level one; the
+    calls checked are exactly FULLRES_CALLS."""
+    _no_experiment_knobs()
+    monkeypatch.setattr(C, "DEFAULT_PRECISION", 0)
+    shadow = _Shadow()
+    shadow.install(monkeypatch)
+    _bench_train_step()
+    assert sorted(shadow.tags) == sorted(FULLRES_CALLS), sorted(shadow.tags)
+    print("\nshadow-checked conv calls: %d (%d distinct tags)" % (sum(shadow.tags.values()), len(shadow.tags)))
+
+
+def test_shadow_check_reports_a_wrong_split():
+    """_Shadow catches a fused backward handed the split planes of another tensor of the same shape (same-size buffer), and passes the
+    right ones"""
+    g = Geo(2, 36, 36, 3, 1, 1, (4, 6, 128))
+    x, w, b, dy = _fullres_operands(g, 67)
+    other = torch.relu(torch.randn_like(x)).contiguous(memory_format=CL3)
+    y = C.conv3d_forward(x, w, b, g.s, g.p, relu=True)
+    shadow = _Shadow()
+    assert shadow.backward(x, dy, y, w, g.s, g.p, True, True, True, precision=0, x_split=_canonical_split(x, 0)) is not None
+    with pytest.raises(AssertionError, match="x_split handed to the backward"):
+        shadow.backward(x, dy, y, w, g.s, g.p, True, True, True, precision=0, x_split=_canonical_split(other, 0))
