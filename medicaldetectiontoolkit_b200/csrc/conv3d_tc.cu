@@ -165,7 +165,13 @@ __device__ __forceinline__ bool tc_step_coords(const TcConvParams &p, int rd, in
 // TPS * CPS * (swz/32) K steps of {1|3} MMAs (split-bf16: A_hi*B_hi, A_hi*B_lo, A_lo*B_hi) into a register accumulator, waits for them,
 // releases the stage, and adds the stage's accumulator into an IEEE fp32 running sum: the tensor core's own accumulation is not
 // round-to-nearest, so no accumulator chain spans more than one stage.
-template <int NT>
+//
+// PLANES > 0: the shape of a stage's batch is fixed at compile time — PLANES (p.planes), KSTEPS (p.swz / 32) and TPS taps of one chunk
+// (p.CPS == 1, p.KW % p.TPS == 0: every tap group is full).  Its descriptors are computed before the fence and its MMAs are issued as one
+// branch-free run between wgmma.fence and the commit.  With run-time trip counts ptxas cannot lay the batch out like that and instead puts
+// a fence of its own in front of almost every MMA.  PLANES == 0: the batch is shaped at run time from p (any plan).  Both issue the same
+// MMAs in the same order (taps, then chunks, then K steps; hi*hi, hi*lo, lo*hi), so their results are bit-identical.
+template <int NT, int PLANES, int KSTEPS, int TPS>
 __global__ void __launch_bounds__(kTcThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcConvParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -255,39 +261,70 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     const int cn = min(p.CPS, p.nchunks - g * p.CPS);
                     for (int kw0 = 0; kw0 < p.KW; kw0 += p.TPS) {
                         mbar_wait(&full[s], ph);
-                        wgmma_fence();
                         const uint32_t sa = smem_base + s * p.stage_bytes, sb = b_base + s * p.stage_bytes;
-                        const int ktaps = min(p.TPS, p.KW - kw0);   // the last tap group of a line may be short
-                        uint32_t scale = 0;                         // the first MMA of a stage overwrites the accumulator
-                        for (int k = 0; k < ktaps; ++k) {
-                            const int shift = p.halo ? (p.dgrad ? p.KW - 1 - (kw0 + k) : kw0 + k) : 0;
-                            for (int c = 0; c < cn; ++c) {
-                                const uint32_t a_hi = sa + c * p.a_chunk_bytes + shift * p.swz;
-                                const uint32_t b_hi = sb + p.a_region_bytes + c * p.b_chunk_bytes + (k * p.planes) * p.b_plane_bytes;
-                                uint64_t da = dtmpl | (uint64_t)((a_hi >> 4) & 0x3FFF);
-                                uint64_t db = dtmpl | (uint64_t)((b_hi >> 4) & 0x3FFF);
-                                uint64_t dal = dtmpl | (uint64_t)(((a_hi + p.a_plane_bytes) >> 4) & 0x3FFF);
-                                uint64_t dbl = dtmpl | (uint64_t)(((b_hi + p.b_plane_bytes) >> 4) & 0x3FFF);
-                                for (int j = 0; j < ksteps; ++j) {
-                                    Wgmma<NT>::template mma<0, 0>(acc, da, db, scale);
-                                    scale = 1;
-                                    if (p.planes > 1) {
-                                        Wgmma<NT>::template mma<0, 0>(acc, da, dbl, 1);
-                                        Wgmma<NT>::template mma<0, 0>(acc, dal, db, 1);
+                        if constexpr (PLANES > 0) {
+                            // descriptors of tap 0; a descriptor is the template plus (address >> 4) < 2^14, so moving the address by
+                            // whole 16-byte units is an add on the descriptor.  Tap k reads the A window shifted by k rows (a_tap: +1 row
+                            // fprop, -1 row dgrad; generic mode: no shift) and B tile k of the stage.
+                            constexpr int swz = 32 * KSTEPS, b_plane = (NT * swz) >> 4;
+                            const int shift0 = p.halo ? (p.dgrad ? p.KW - 1 - kw0 : kw0) : 0;
+                            const long long a_tap = p.halo ? (p.dgrad ? -(swz >> 4) : (swz >> 4)) : 0;
+                            const uint64_t da0 = dtmpl | (uint64_t)(((sa + shift0 * swz) >> 4) & 0x3FFF);
+                            const uint64_t db0 = dtmpl | (uint64_t)(((sb + p.a_region_bytes) >> 4) & 0x3FFF);
+                            const uint64_t a_lo = (uint64_t)(p.a_plane_bytes >> 4);
+                            wgmma_fence();
+#pragma unroll
+                            for (int k = 0; k < TPS; ++k) {
+                                const uint64_t da = da0 + (uint64_t)(k * a_tap), db = db0 + (uint64_t)(k * PLANES * b_plane);
+#pragma unroll
+                                for (int j = 0; j < KSTEPS; ++j) {   // +32 bytes along K per step
+                                    // the first MMA of a stage overwrites the accumulator (scale_d = 0, a compile-time constant)
+                                    Wgmma<NT>::template mma<0, 0>(acc, da + 2 * j, db + 2 * j, (k == 0 && j == 0) ? 0u : 1u);
+                                    if constexpr (PLANES > 1) {
+                                        Wgmma<NT>::template mma<0, 0>(acc, da + 2 * j, db + b_plane + 2 * j, 1);
+                                        Wgmma<NT>::template mma<0, 0>(acc, da + a_lo + 2 * j, db + 2 * j, 1);
                                     }
-                                    da += 2; db += 2; dal += 2; dbl += 2;          // +32 bytes along K
                                 }
                             }
+                        } else {
+                            const int ktaps = min(p.TPS, p.KW - kw0);   // the last tap group of a line may be short
+                            uint32_t scale = 0;                         // the first MMA of a stage overwrites the accumulator
+                            // ktaps, cn and ksteps are >= 1: the loops test at the bottom, so that no path reaches the commit around the MMAs
+                            int k = 0;
+                            do {
+                                const int shift = p.halo ? (p.dgrad ? p.KW - 1 - (kw0 + k) : kw0 + k) : 0;
+                                int c = 0;
+                                do {
+                                    const uint32_t a_hi = sa + c * p.a_chunk_bytes + shift * p.swz;
+                                    const uint32_t b_hi = sb + p.a_region_bytes + c * p.b_chunk_bytes + (k * p.planes) * p.b_plane_bytes;
+                                    uint64_t da = dtmpl | (uint64_t)((a_hi >> 4) & 0x3FFF);
+                                    uint64_t db = dtmpl | (uint64_t)((b_hi >> 4) & 0x3FFF);
+                                    uint64_t dal = dtmpl | (uint64_t)(((a_hi + p.a_plane_bytes) >> 4) & 0x3FFF);
+                                    uint64_t dbl = dtmpl | (uint64_t)(((b_hi + p.b_plane_bytes) >> 4) & 0x3FFF);
+                                    int j = 0;
+                                    do {
+                                        wgmma_fence();   // run-time trip counts: a fence per K step, where ptxas would otherwise insert its own
+                                        Wgmma<NT>::template mma<0, 0>(acc, da, db, scale);
+                                        scale = 1;
+                                        if (p.planes > 1) {
+                                            wgmma_fence();
+                                            Wgmma<NT>::template mma<0, 0>(acc, da, dbl, 1);
+                                            Wgmma<NT>::template mma<0, 0>(acc, dal, db, 1);
+                                        }
+                                        da += 2; db += 2; dal += 2; dbl += 2;          // +32 bytes along K
+                                    } while (++j < ksteps);
+                                } while (++c < cn);
+                            } while (++k < ktaps);
+                            wgmma_fence();   // the loops merge here: ptxas wants a fence before the commit as well
                         }
                         wgmma_commit();
                         wgmma_wait<0>();
                         reg_fence<NT / 2>(acc);
                         __syncwarp();
                         if (lane == 0) mbar_arrive(&empty[s]);
-                        if (scale) {
+                        // every stage issues at least one MMA (ktaps >= 1, cn >= 1), so its accumulator always holds the stage's sum
 #pragma unroll
-                            for (int i = 0; i < NT / 2; ++i) sum[i] += acc[i];
-                        }
+                        for (int i = 0; i < NT / 2; ++i) sum[i] += acc[i];
                         if (++s == p.D) { s = 0; ph ^= 1; }
                     }
                 }
@@ -371,13 +408,22 @@ size_t conv_tc_workspace_bytes(const ConvGeom &g, int pass, int precision) {
     return align_up((size_t)planes * pl.src_rows * pl.Kg * 2, 1024) + align_up((size_t)planes * T * pl.Np * pl.Kp * 2, 1024) + 2048;
 }
 
-template <int NT>
+template <int NT, int PLANES = 0, int KSTEPS = 0, int TPS = 0>
 static int launch_tc(dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap &tmA, const CUtensorMap &tmB, const TcConvParams &p) {
     static bool attr[kMaxDevices] = {};
-    if (!ensure_smem_attr(conv_tc_kernel<NT>, 220 * 1024, attr)) return MDT_EDRIVER;
-    conv_tc_kernel<NT><<<grid, kTcThreads, smem, st>>>(tmA, tmB, p);
+    if (!ensure_smem_attr(conv_tc_kernel<NT, PLANES, KSTEPS, TPS>, 220 * 1024, attr)) return MDT_EDRIVER;
+    conv_tc_kernel<NT, PLANES, KSTEPS, TPS><<<grid, kTcThreads, smem, st>>>(tmA, tmB, p);
     return launch_status();
 }
+
+// (NT, K steps per chunk, taps per stage) of the stage batches compiled with a fixed shape, at both precisions: the plans of the Retina U-Net
+// train step's convs — halo-line layers (3 or 7 taps per stage) and generic-mode and 1x1x1 layers (one tap per stage).  Other plans run
+// the run-time-shaped batch.
+#define MDT_TC_FIXED_SHAPES(X)                                  \
+    X(32, 2, 3) X(32, 2, 7) X(32, 4, 1) X(32, 4, 3)             \
+    X(48, 4, 1) X(48, 4, 3)                                     \
+    X(64, 2, 1) X(64, 2, 3) X(64, 4, 1) X(64, 4, 3)             \
+    X(80, 4, 1) X(128, 4, 1)
 
 // presplit != nullptr: the A operand is already in split form (layout of split_rows_kernel with inter_w = SW) and `src` is ignored
 int conv_tc_run(const ConvGeom &g, int pass, const float *src, const float *w, const float *bias, const float *residual, float *dst,
@@ -440,6 +486,13 @@ int conv_tc_run(const ConvGeom &g, int pass, const float *src, const float *w, c
 
     const size_t smem = (size_t)p.D * p.stage_bytes + 1024;
     const dim3 grid((unsigned)((long long)g.n * pl.RD * p.tiles_h * p.tiles_w), pl.n_tiles_n);
+    if (p.CPS == 1 && g.kw % p.TPS == 0) {   // every stage holds TPS taps of one chunk
+#define MDT_TC_FIXED(NT_, KS, TPS_)                                                                                       \
+        if (pl.NT == NT_ && pl.swz == 32 * KS && p.TPS == TPS_)                                                          \
+            return planes == 2 ? launch_tc<NT_, 2, KS, TPS_>(grid, smem, st, tmA, tmB, p) : launch_tc<NT_, 1, KS, TPS_>(grid, smem, st, tmA, tmB, p);
+        MDT_TC_FIXED_SHAPES(MDT_TC_FIXED)
+#undef MDT_TC_FIXED
+    }
     switch (pl.NT) {
         case 16: return launch_tc<16>(grid, smem, st, tmA, tmB, p);
         case 32: return launch_tc<32>(grid, smem, st, tmA, tmB, p);

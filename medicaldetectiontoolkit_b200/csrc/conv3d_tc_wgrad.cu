@@ -63,7 +63,12 @@ __device__ __forceinline__ void wg_decode_cb(const TcWgradParams &p, int cb, int
     kd = pair / p.KH;
 }
 
-template <int NC>   // accumulator columns per column block = KW * chunkx
+// NC: accumulator columns per column block = KW * chunkx.
+// KSTEPS > 0: the shape of a unit's MMA batch is fixed at compile time — PLANES (p.planes), MTRICK (p.mtrick), KSTEPS (p.ksteps) and the
+// descriptor steps along K, SWY (p.swy) and SWX (p.swx) — and the batch is one branch-free run of MMAs between wgmma.fence and the commit.
+// KSTEPS == 0: the batch is shaped at run time from p (any plan).  Both issue the same MMAs in the same order, so their results are
+// bit-identical.
+template <int NC, int PLANES, int MTRICK, int KSTEPS, int SWY, int SWX>
 __global__ void __launch_bounds__(kWgThreads, 1)
 conv_tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_constant__ CUtensorMap tmX, const TcWgradParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -134,20 +139,40 @@ conv_tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_const
             const int s = it % p.stages;
             mbar_wait(&full[s], (it / p.stages) & 1);
             if (live && (!p.ksplit || (it & 1) == wg) && p.skip != 1) {
-                wgmma_fence();
                 const uint32_t y_hi = smem_u32(smem + (size_t)s * p.stage_bytes) + y_wg;
                 const uint32_t x0 = smem_u32(smem + (size_t)s * p.stage_bytes + p.x_base);
                 uint64_t dyh = ytmpl | (uint64_t)((y_hi >> 4) & 0x3FFF);
                 uint64_t dyl = ytmpl | (uint64_t)(((y_hi + p.y_plane_bytes) >> 4) & 0x3FFF);
                 uint64_t dxh = xtmpl | (uint64_t)((x0 >> 4) & 0x3FFF);
                 uint64_t dxl = xtmpl | (uint64_t)(((x0 + p.x_plane_bytes) >> 4) & 0x3FFF);
-                for (int k = 0; k < p.ksteps; ++k) {
-                    Wgmma<NC>::template mma<1, 1>(acc, dyh, dxh, 1);
-                    if (p.planes > 1) {
-                        Wgmma<NC>::template mma<1, 1>(acc, dyh, dxl, 1);
-                        if (!p.mtrick) Wgmma<NC>::template mma<1, 1>(acc, dyl, dxh, 1);
+                if constexpr (KSTEPS > 0) {
+                    wgmma_fence();
+#pragma unroll
+                    for (int k = 0; k < KSTEPS; ++k) {   // 16 voxel rows further along K per step: (16 * swizzle bytes) >> 4
+                        Wgmma<NC>::template mma<1, 1>(acc, dyh + k * SWY, dxh + k * SWX, 1);
+                        if constexpr (PLANES > 1) {
+                            Wgmma<NC>::template mma<1, 1>(acc, dyh + k * SWY, dxl + k * SWX, 1);
+                            if constexpr (!MTRICK) Wgmma<NC>::template mma<1, 1>(acc, dyl + k * SWY, dxh + k * SWX, 1);
+                        }
                     }
-                    dyh += ystep; dyl += ystep; dxh += xstep; dxl += xstep;     // 16 voxel rows further along K
+                } else {
+                    // p.ksteps >= 1: the loop tests at the bottom; with run-time trip counts a fence per K step and one before the commit,
+                    // where ptxas would otherwise insert its own
+                    int k = 0;
+                    do {
+                        wgmma_fence();
+                        Wgmma<NC>::template mma<1, 1>(acc, dyh, dxh, 1);
+                        if (p.planes > 1) {
+                            wgmma_fence();
+                            Wgmma<NC>::template mma<1, 1>(acc, dyh, dxl, 1);
+                            if (!p.mtrick) {
+                                wgmma_fence();
+                                Wgmma<NC>::template mma<1, 1>(acc, dyl, dxh, 1);
+                            }
+                        }
+                        dyh += ystep; dyl += ystep; dxh += xstep; dxl += xstep;     // 16 voxel rows further along K
+                    } while (++k < p.ksteps);
+                    wgmma_fence();
                 }
                 wgmma_commit();
                 wgmma_wait<0>();
@@ -285,12 +310,36 @@ size_t conv_tc_wgrad_workspace_bytes(const ConvGeom &g, int precision) {
            wg_align(conv_bias_grad_ws_bytes(g)) + 2048;
 }
 
-template <int NC>
+template <int NC, int PLANES = 0, int MTRICK = 0, int KSTEPS = 0, int SWY = 0, int SWX = 0>
 static int launch_wgrad(dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap &tmY, const CUtensorMap &tmX, const TcWgradParams &p) {
     static bool attr[kMaxDevices] = {};
-    if (!ensure_smem_attr(conv_tc_wgrad_kernel<NC>, 220 * 1024, attr)) return MDT_EDRIVER;
-    conv_tc_wgrad_kernel<NC><<<grid, kWgThreads, smem, st>>>(tmY, tmX, p);
+    if (!ensure_smem_attr(conv_tc_wgrad_kernel<NC, PLANES, MTRICK, KSTEPS, SWY, SWX>, 220 * 1024, attr)) return MDT_EDRIVER;
+    conv_tc_wgrad_kernel<NC, PLANES, MTRICK, KSTEPS, SWY, SWX><<<grid, kWgThreads, smem, st>>>(tmY, tmX, p);
     return launch_status();
+}
+
+// (NC, mtrick, K steps, dy swizzle bytes, x swizzle bytes) of the unit batches compiled with a fixed shape, at both precisions: the plans
+// of the Retina U-Net train step's weight gradients with K steps >= 4 (output lines of >= 64 voxels).  Other plans run the run-time-shaped
+// batch.
+#define MDT_WG_FIXED_SHAPES(X)                                                                    \
+    X(96, 1, 8, 64, 64) X(224, 1, 8, 64, 64) X(192, 1, 8, 128, 128) X(192, 1, 8, 64, 128)         \
+    X(192, 1, 4, 128, 128) X(192, 1, 4, 64, 128) X(64, 1, 4, 128, 128) X(64, 0, 4, 128, 128)
+
+static int launch_wgrad_plan(const ConvGeom &g, const WgPlan &w, int planes, dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap &tmY,
+                             const CUtensorMap &tmX, const TcWgradParams &p) {
+#define MDT_WG_FIXED(NC, MT, KS, SY, SX)                                                                     \
+    if (g.kw * w.chunkx == NC && w.mtrick == MT && w.ksteps == KS && w.swy == SY && w.swx == SX)            \
+        return planes == 2 ? launch_wgrad<NC, 2, MT, KS, SY, SX>(grid, smem, st, tmY, tmX, p)               \
+                           : launch_wgrad<NC, 1, MT, KS, SY, SX>(grid, smem, st, tmY, tmX, p);
+    MDT_WG_FIXED_SHAPES(MDT_WG_FIXED)
+#undef MDT_WG_FIXED
+    switch (g.kw * w.chunkx) {
+#define MDT_WG_CASE(N) case N: return launch_wgrad<N>(grid, smem, st, tmY, tmX, p);
+        MDT_WG_CASE(16) MDT_WG_CASE(32) MDT_WG_CASE(48) MDT_WG_CASE(64) MDT_WG_CASE(80) MDT_WG_CASE(96) MDT_WG_CASE(112) MDT_WG_CASE(128)
+        MDT_WG_CASE(144) MDT_WG_CASE(160) MDT_WG_CASE(176) MDT_WG_CASE(192) MDT_WG_CASE(208) MDT_WG_CASE(224) MDT_WG_CASE(240) MDT_WG_CASE(256)
+#undef MDT_WG_CASE
+        default: return MDT_EUNSUPPORTED;
+    }
 }
 
 // dy_presplit != nullptr: dy is already split (interleaved layout, conv_tc_kpad(cout) channels); then db must have been produced by the caller
@@ -363,14 +412,7 @@ static int conv_tc_wgrad_impl(const ConvGeom &g, const float *x, const float *dy
     const size_t smem = (size_t)p.stages * p.stage_bytes + 1024 + tail;
     if (smem > 218 * 1024) return MDT_EUNSUPPORTED;
     const dim3 grid((unsigned)(w.groups * p.splits), w.mtiles);
-    switch (g.kw * w.chunkx) {
-#define MDT_WG_CASE(N) case N: rc = launch_wgrad<N>(grid, smem, st, tmY, tmX, p); break;
-        MDT_WG_CASE(16) MDT_WG_CASE(32) MDT_WG_CASE(48) MDT_WG_CASE(64) MDT_WG_CASE(80) MDT_WG_CASE(96) MDT_WG_CASE(112) MDT_WG_CASE(128)
-        MDT_WG_CASE(144) MDT_WG_CASE(160) MDT_WG_CASE(176) MDT_WG_CASE(192) MDT_WG_CASE(208) MDT_WG_CASE(224) MDT_WG_CASE(240) MDT_WG_CASE(256)
-#undef MDT_WG_CASE
-        default: rc = MDT_EUNSUPPORTED;
-    }
-    if (rc) return rc;
+    if ((rc = launch_wgrad_plan(g, w, planes, grid, smem, st, tmY, tmX, p))) return rc;
     {
         const long long total = (long long)g.cout * w.ncb_total * g.kw * w.chunkx;
         wgrad_reduce_kernel<<<(unsigned)ceil_div<long long>(total, 256), 256, 0, st>>>(p, dw);
