@@ -75,9 +75,11 @@ def roi_ap(score, seg, kind, n_seg, thresholds, recall_points):
     q = np.zeros((n_seg, n_thr, n_r))
     counts = np.zeros((n_seg, 1 + n_thr), dtype=np.int32)
     counts[:, 0] = np.bincount(seg[(seg >= 0) & ((kind == 0) | (kind == 2))], minlength=n_seg)
-    ranked = (seg >= 0) & ((kind == 0) | (kind == 1)) & ~np.isnan(score)
+    ranked = np.nonzero((seg >= 0) & ((kind == 0) | (kind == 1)) & ~np.isnan(score))[0]
+    ranked = ranked[np.argsort(seg[ranked], kind='stable')]          # grouped by segment once, each group in row order
+    bounds = np.searchsorted(seg[ranked], np.arange(n_seg + 1))
     for s in range(n_seg):
-        idx = np.nonzero(ranked & (seg == s))[0]
+        idx = ranked[bounds[s]:bounds[s + 1]]
         idx = idx[np.argsort(-score[idx], kind='stable')]
         ss = score[idx]
         tpc = np.cumsum(kind[idx] == 0)
