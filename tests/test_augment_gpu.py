@@ -38,7 +38,8 @@ def test_elastic_field_vs_gaussian_filter(dim, shape, sigma):
     for b in range(2):
         for d in range(dim):
             ref = gaussian_filter(nz[b, d], sigma if b == 0 else sigma * 0.9, mode='constant', cval=0)
-            assert np.abs(got[b, d] - ref).max() <= 1e-5 * np.abs(ref).max()
+            # fp64 weights and accumulation, as scipy: the two differ only by summation order and the device's exp (about 3e-15)
+            assert np.abs(got[b, d] - ref).max() <= 1e-12 * np.abs(ref).max()
     scaled = A.elastic_field(noise, [sigma, sigma * 0.9], [1500.0, 7.0]).cpu().numpy()
     assert np.array_equal(scaled[0], got[0] * 1500.0) and np.array_equal(scaled[1], got[1] * 7.0)
 
@@ -255,19 +256,19 @@ def test_augmenter_end_to_end(dim):
     out = A.Augmenter(cf, seed=6, rank=0, with_masks=True)(batch)
     want = _oracle_batch(cf, batch, 6, True)
     assert out['data'].dtype == torch.float32 and out['data'].is_cuda and out['seg'].dtype == torch.uint8
-    # data: the elastic field's own 1e-5 error moves the 2D coordinates, so the bound there is looser
-    tol = (1e-5 if dim == 3 else 2e-3) * np.abs(batch['data']).max()
+    # data: the 2D elastic field agrees with scipy's to about 1e-15 of its size, so it moves the coordinates by far less than the fp32
+    # spline's own error and both dims meet the same bound
+    tol = 1e-5 * np.abs(batch['data']).max()
     assert np.abs(out['data'].cpu().numpy() - want['data']).max() <= tol
     gseg = out['seg'].cpu().numpy()
-    if dim == 3:
-        # no elastic field in 3D: the seg, and with it every box, label and mask, equal the oracle's except at rounding boundaries
-        near = np.stack([_near_boundary(c, src) for c in want['coords']])[:, None]
-        assert not ((gseg != want['seg']) & ~near).any()
-        if not ((gseg != want['seg']) & near).any():
-            for b in range(3):
-                assert np.array_equal(np.asarray(out['bb_target'][b]), np.asarray(want['bb_target'][b]))
-                assert np.array_equal(out['roi_labels'][b], want['roi_labels'][b])
-                assert np.array_equal(out['roi_masks'][b], want['roi_masks'][b])
+    # the seg, and with it every box, label and mask, equal the oracle's except at rounding boundaries
+    near = np.stack([_near_boundary(c, src) for c in want['coords']])[:, None]
+    assert not ((gseg != want['seg']) & ~near).any()
+    if not ((gseg != want['seg']) & near).any():
+        for b in range(3):
+            assert np.array_equal(np.asarray(out['bb_target'][b]), np.asarray(want['bb_target'][b]))
+            assert np.array_equal(out['roi_labels'][b], want['roi_labels'][b])
+            assert np.array_equal(out['roi_masks'][b], want['roi_masks'][b])
     # always: boxes / labels / masks / relabelled seg equal the oracle applied to the op's own warped instance map
     raw = _raw_warp(cf, batch, 6)
     ref = O.seg_to_boxes(raw, batch['class_target'], dim, True)
