@@ -392,6 +392,34 @@ int mdt_eval_patient(const double *row_score, const int *row_label, const int *r
                      const int *seg_slots, int n_members, int n_seg, double *thr, int *tps, int *fps, int *n_thr, void *ws, size_t ws_bytes,
                      void *stream);
 
+/* ------------------------------------------------------------- data loader (csrc/loader.cu) -----------------------------------------------
+ * replaces: the volume scans of BatchGenerator.generate_train_batch and the tiling of PatientBatchIterator.generate_train_batch in
+ * experiments/{lidc_exp,toy_exp,pet_ct_tnm_classification}/data_loader.py (np.sum / np.unique / np.argwhere over the whole patient, np.pad,
+ * np.take, the slice and patch crops).
+ *
+ * mdt_loader_fg_index: seg [z, y, x] uint8, one patient in the memory order of its .npy file, read as the transposed (y, x, z) view the
+ * loaders work on.  counts [256] int32 = voxels per label (counts[0]: background).  order [cap] int32 = the (y, x, z) linear index
+ * (y * x_ext + x) * z_ext + z of every foreground voxel, grouped by label (1 .. 255 ascending), each group in ascending index order (np.argwhere
+ * of seg == label on the transposed view); entries at or past min(cap, number of foreground voxels) are not written.  cap = 0 (order may be
+ * NULL) writes counts only.  z <= 6000 and z * y * x < 2^31, else MDT_EUNSUPPORTED.  Deterministic.  Workspace: 1 KiB per 32-column tile of
+ * a y row. */
+size_t mdt_loader_fg_index_workspace_bytes(int z, int y, int x);
+int mdt_loader_fg_index(const unsigned char *seg, int z, int y, int x, int *counts, int *order, int cap, void *ws, size_t ws_bytes, void *stream);
+/* mdt_loader_gather: out [n, c, i, j, k] (out_dtype) = src_b[tab_c[b, c], tab_z[b, c, k], tab_y[b, i], tab_x[b, j]] where src_b is element
+ * b's [c, z, y, x] volume (src_dtype) at element offset elems[b].offset of src; a table entry outside [0, extent) of its axis (-1 by
+ * convention) gives 0.  Converts as numpy's astype does (float -> uint8 truncates; fp64 -> fp16 rounds once).  k > 1: i <= 65535 and n * c <=
+ * 65535, else MDT_EUNSUPPORTED.  Tables are device int32 arrays.  No workspace. */
+#define MDT_DTYPE_U8 0
+#define MDT_DTYPE_F16 1
+#define MDT_DTYPE_F32 2
+#define MDT_DTYPE_F64 3
+typedef struct mdt_loader_src {
+    long long offset;  /* in elements of src_dtype */
+    int c, z, y, x;    /* the element's source extents */
+} mdt_loader_src;
+int mdt_loader_gather(int src_dtype, const void *src, const mdt_loader_src *elems, int n, int c, int i, int j, int k, const int *tab_c, const int *tab_z,
+                      const int *tab_y, const int *tab_x, int out_dtype, void *out, void *stream);
+
 /* number of kernel launches issued by this library since load (all entry points) — feeds bench.py's gpu_launches */
 unsigned long long mdt_launch_count(void);
 

@@ -110,6 +110,9 @@ SIGNATURES = {
     "mdt_eval_patient_workspace_bytes": (_SZ, [_I, _I]),
     "mdt_eval_patient": (_I, [_VP, _VP, _VP, _I, _I, _VP, _VP, _I, _I, _VP, _VP, _VP, _VP, _VP, _SZ, _VP]),
     "mdt_unmold_masks": (_I, [_I, _VP, _I, _VP, c_i64p, _I, ctypes.POINTER(_I), _I, ctypes.POINTER(_I), _VP, _VP, _VP]),
+    "mdt_loader_fg_index_workspace_bytes": (_SZ, [_I, _I, _I]),
+    "mdt_loader_fg_index": (_I, [_VP, _I, _I, _I, _VP, _VP, _I, _VP, _SZ, _VP]),
+    "mdt_loader_gather": (_I, [_I, _VP, _VP, _I, _I, _I, _I, _I, _VP, _VP, _VP, _VP, _I, _VP, _VP]),
 }
 
 

@@ -183,6 +183,31 @@ def make_cf(model='retina_unet', dim=3, patch_size=None, exp='lidc_exp', batch_s
         cf.learning_rate = [1e-4] * 50 + [5 * 1e-5] * 25 + [1e-5] * 25
         cf.return_masks_in_test = False
         cf.n_plot_rpn_props = 5 if dim == 2 else 30
+    # data loader (data_loader.py; experiments/*/configs.py and default_configs.py, outside server_env).  The dataset paths and cf.exp_dir
+    # are the user's to set.
+    cf.experiment = exp
+    if not hasattr(cf, 'pre_crop_size'):
+        if exp == 'lidc_exp':
+            cf.pre_crop_size = [300, 300] if dim == 2 else [156, 156, 96]
+        elif dim == 2:
+            cf.pre_crop_size = [320, 320]
+    cf.seed = 0
+    cf.server_env = False
+    cf.input_df_name = 'info_df.pickle'
+    cf.pp_data_path = cf.pp_test_data_path = cf.exp_dir = None
+    cf.created_fold_id_pickle = False
+    cf.hold_out_test_set = exp != 'lidc_exp'
+    cf.select_prototype_subset = 100 if exp == 'lidc_exp' else None
+    cf.batch_sample_slack = 0.2
+    cf.n_3D_context = None
+    cf.merge_2D_to_3D_preds = exp != 'toy_exp'
+    cf.val_mode = 'val_patient' if exp == 'toy_exp' else 'val_sampling'
+    cf.max_val_patients = None if exp == 'toy_exp' else 50
+    cf.num_val_batches = 10 if exp == PETCT else 50
+    cf.max_test_patients = 'all'
+    cf.n_workers = 8
+    if exp == 'toy_exp':
+        cf.n_train_val_data = 1500
     return cf
 
 
