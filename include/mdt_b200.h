@@ -413,12 +413,39 @@ int mdt_loader_fg_index(const unsigned char *seg, int z, int y, int x, int *coun
 #define MDT_DTYPE_F16 1
 #define MDT_DTYPE_F32 2
 #define MDT_DTYPE_F64 3
+#define MDT_DTYPE_I16 4
 typedef struct mdt_loader_src {
     long long offset;  /* in elements of src_dtype */
     int c, z, y, x;    /* the element's source extents */
 } mdt_loader_src;
 int mdt_loader_gather(int src_dtype, const void *src, const mdt_loader_src *elems, int n, int c, int i, int j, int k, const int *tab_c, const int *tab_z,
                       const int *tab_y, const int *tab_x, int out_dtype, void *out, void *stream);
+
+/* ------------------------------------------------------------- LIDC preprocessing (csrc/preprocess.cu) ------------------------------------
+ * replaces: the skimage.transform.resize calls (scikit-image 0.16.2: order 1, mode 'edge', anti_aliasing on, clip) and the numpy CT
+ * normalisation and rater vote of experiments/lidc_exp/preprocessing.py (resample_array, pp_patient).  Volumes are (z, y, x), C order.
+ * Every call is asynchronous on `stream` and deterministic (no atomics).
+ *
+ * mdt_pp_resample: out [out_shape] fp32 = resize(src [in_shape] as fp64): with factors f = in / out per axis, scipy's gaussian_filter at
+ * sigma = max(0, (f - 1) / 2) with mode 'nearest' on the axes with sigma > 1e-15 (fp64 weights, radius int(4 sigma + 0.5) <= 64, else
+ * MDT_EUNSUPPORTED), then map_coordinates(order=1, mode='nearest') at f (j + 0.5) - 0.5 in fp64, rounded once to fp32.  src_dtype:
+ * MDT_DTYPE_U8, MDT_DTYPE_I16 or MDT_DTYPE_F32.  Workspace: one fp64 volume of in_shape per blurred axis, at most two (0 bytes when no
+ * axis is blurred, ws may then be NULL). */
+size_t mdt_pp_resample_workspace_bytes(const int *in_shape, const int *out_shape);
+int mdt_pp_resample(int src_dtype, const void *src, const int *in_shape, const int *out_shape, float *out, void *ws, size_t ws_bytes, void *stream);
+/* mdt_pp_normalize: x [n] fp32 in place: clip to [-1200, 600], mean and population std of the clipped values in fp64 (fixed 1024-way
+ * partial sums and fixed trees), then x = fl32(fl32(x - fl32(mean)) / fp16(fl32(std))).  stats [2] fp64 (device) = {mean, std} before
+ * rounding.  Workspace: 8 KiB. */
+size_t mdt_pp_normalize_workspace_bytes(long long n);
+int mdt_pp_normalize(float *x, long long n, double *stats, void *ws, size_t ws_bytes, void *stream);
+/* mdt_pp_vote_add: acc [n] fp32 = first ? rater : acc + rater (the raters of one ROI summed in fp32 in call order). */
+int mdt_pp_vote_add(float *acc, const float *rater, long long n, int first, void *stream);
+/* mdt_pp_vote_label: the vote of ROI `roi` (0-based, <= 254, else MDT_EUNSUPPORTED): where acc / max(4, n_raters) >= 0.5 (fp32 division),
+ * labels [n] uint8 = 1 + the number of ROIs r < roi with kept[r] != 0; kept [>= roi + 1] int32: kept[roi] = 1 if any voxel was labelled, else
+ * 0 (kept[0 .. roi) are read).  roi 0 writes every voxel of labels (0 where its vote is below 0.5); later ROIs overwrite. */
+int mdt_pp_vote_label(const float *acc, long long n, int n_raters, int roi, unsigned char *labels, int *kept, void *stream);
+/* mdt_pp_label_summary: labels [z, plane] uint8 -> slice_nz [z] uint8 = any voxel of the slice != 0, present [256] uint8 = label occurs. */
+int mdt_pp_label_summary(const unsigned char *labels, int z, long long plane, unsigned char *slice_nz, unsigned char *present, void *stream);
 
 /* number of kernel launches issued by this library since load (all entry points) — feeds bench.py's gpu_launches */
 unsigned long long mdt_launch_count(void);

@@ -113,6 +113,13 @@ SIGNATURES = {
     "mdt_loader_fg_index_workspace_bytes": (_SZ, [_I, _I, _I]),
     "mdt_loader_fg_index": (_I, [_VP, _I, _I, _I, _VP, _VP, _I, _VP, _SZ, _VP]),
     "mdt_loader_gather": (_I, [_I, _VP, _VP, _I, _I, _I, _I, _I, _VP, _VP, _VP, _VP, _I, _VP, _VP]),
+    "mdt_pp_resample_workspace_bytes": (_SZ, [ctypes.POINTER(_I), ctypes.POINTER(_I)]),
+    "mdt_pp_resample": (_I, [_I, _VP, ctypes.POINTER(_I), ctypes.POINTER(_I), _VP, _VP, _SZ, _VP]),
+    "mdt_pp_normalize_workspace_bytes": (_SZ, [_I64]),
+    "mdt_pp_normalize": (_I, [_VP, _I64, _VP, _VP, _SZ, _VP]),
+    "mdt_pp_vote_add": (_I, [_VP, _VP, _I64, _I, _VP]),
+    "mdt_pp_vote_label": (_I, [_VP, _I64, _I, _I, _VP, _VP, _VP]),
+    "mdt_pp_label_summary": (_I, [_VP, _I, _I64, _VP, _VP, _VP]),
 }
 
 
