@@ -447,6 +447,20 @@ int mdt_pp_vote_label(const float *acc, long long n, int n_raters, int roi, unsi
 /* mdt_pp_label_summary: labels [z, plane] uint8 -> slice_nz [z] uint8 = any voxel of the slice != 0, present [256] uint8 = label occurs. */
 int mdt_pp_label_summary(const unsigned char *labels, int z, long long plane, unsigned char *slice_nz, unsigned char *present, void *stream);
 
+/* ------------------------------------------------------------- toy experiment images (csrc/toys.cu) ----------------------------------------
+ * replaces: multi_processing_create_image of experiments/toy_exp/generate_toys.py, with a per-image seed in place of numpy's global state.
+ *
+ * mdt_toy_images: image b draws from numpy's legacy RandomState seeded by init_by_array on keys [b, 0 .. 2] (device uint32 [n, 3]), with
+ * the reference's calls in its order: rand(320, 320), then cx = randint(margin, 320 - margin), cy = randint(margin, 320 - margin),
+ * class_id = randint(0, 2).  Where (x - cx)^2 + (y - cy)^2 < r^2 (x the column, y the row, r = radius0 / radius1 by class_id) it adds 0.2
+ * to the image and sets seg to 1; with MDT_TOY_HOLE and class_id 1 it then subtracts 0.2 where the distance is below 4, and with
+ * MDT_TOY_HOLE_CLEARS_SEG also sets seg to 0 there.  img: device fp64 [n, 2, 320, 320] (image plane, then seg as 0.0 / 1.0), the array the
+ * reference saves; params: device int32 [n, 3] = (cx, cy, class_id).  0 <= margin < 320 - margin, radii >= 0, else MDT_EINVAL.  One CTA per
+ * image; the bound is the 1.64 MB written per image and the 329 dependent twists of its MT19937 state.  No workspace; deterministic. */
+#define MDT_TOY_HOLE 1
+#define MDT_TOY_HOLE_CLEARS_SEG 2
+int mdt_toy_images(const uint32_t *keys, int n, int margin, int radius0, int radius1, int flags, double *img, int *params, void *stream);
+
 /* number of kernel launches issued by this library since load (all entry points) — feeds bench.py's gpu_launches */
 unsigned long long mdt_launch_count(void);
 

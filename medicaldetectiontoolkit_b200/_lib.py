@@ -120,6 +120,7 @@ SIGNATURES = {
     "mdt_pp_vote_add": (_I, [_VP, _VP, _I64, _I, _VP]),
     "mdt_pp_vote_label": (_I, [_VP, _I64, _I, _I, _VP, _VP, _VP]),
     "mdt_pp_label_summary": (_I, [_VP, _I, _I64, _VP, _VP, _VP]),
+    "mdt_toy_images": (_I, [_VP, _I, _I, _I, _I, _I, _VP, _VP, _VP]),
 }
 
 
