@@ -447,6 +447,52 @@ int mdt_pp_vote_label(const float *acc, long long n, int n_raters, int roi, unsi
 /* mdt_pp_label_summary: labels [z, plane] uint8 -> slice_nz [z] uint8 = any voxel of the slice != 0, present [256] uint8 = label occurs. */
 int mdt_pp_label_summary(const unsigned char *labels, int z, long long plane, unsigned char *slice_nz, unsigned char *present, void *stream);
 
+/* ------------------------------------------------------------- PET-CT preprocessing (csrc/petct_preprocess.cu) -----------------------------
+ * replaces: the SimpleITK resampling, the segment merge, get_z_crops' per-slice scan (clear_border, scipy.ndimage.label, center_of_mass) and
+ * the two-channel normalisation of experiments/pet_ct_tnm_classification/preprocessing.py.  Volumes are (z, y, x), C order, unless strides
+ * say otherwise.  Every call is asynchronous on `stream` and deterministic.
+ *
+ * mdt_petct_grid: an ITK image geometry in ITK's (x, y, z) axis order: size, origin, spacing (> 0) and the row-major 3x3 direction.
+ * mdt_petct_resample: out (out_grid) = ResampleImageFilter of src (in_grid) with the identity transform and linear interpolation, per voxel in
+ * fp64: p = origin_o + sum_c (direction_o[r][c] spacing_o[c]) i_c, then c_r = sum_k (direction_i[k][r] / spacing_i[r]) (p_k - origin_i[k]),
+ * each sum taken in axis order without contraction.  A point with some c_r outside [-0.5, size_r - 0.5) gets 0; otherwise base = max(0,
+ * floor(c)), and per axis (x, then y, then z) a + (b - a) d with d = c - base (the base sample alone where d <= 0 or base + 1 is past the
+ * end).  The value is clamped to out_dtype's range and truncated (MDT_DTYPE_U8, MDT_DTYPE_I16) or rounded (MDT_DTYPE_F32).  src_dtype and
+ * out_dtype: MDT_DTYPE_U8, MDT_DTYPE_I16 or MDT_DTYPE_F32, else MDT_EINVAL.  No workspace. */
+typedef struct mdt_petct_grid {
+    int size[3];
+    double origin[3];
+    double spacing[3];
+    double direction[9];
+} mdt_petct_grid;
+int mdt_petct_resample(int src_dtype, const void *src, const mdt_petct_grid *in_grid, int out_dtype, void *out, const mdt_petct_grid *out_grid,
+                       void *stream);
+/* mdt_petct_seg_merge: out [z, y, x] uint8 = 1 where some segment k with selected[k] != 0 (host uint8 [n_seg]) has segs[k, x, y, z] == 1,
+ * else 0.  segs: device, src_dtype as for mdt_petct_resample, element strides (host int64 [4], >= 0) of its axes (k, x, y, z).  n_seg <= 256,
+ * else MDT_EUNSUPPORTED.  No workspace. */
+int mdt_petct_seg_merge(int src_dtype, const void *segs, int n_seg, int x, int y, int z, const long long *strides, const unsigned char *selected,
+                        unsigned char *out, void *stream);
+/* mdt_petct_body_components: per z slice of ct [z, y, x] (src_dtype as above), the pixels with value < -600, without the 8-connected
+ * components that own a pixel of the slice's one-pixel border (skimage's clear_border), labelled with 4-connectivity (scipy.ndimage.label)
+ * and numbered over the volume in C order of their first pixel.  label [z, y, x] int32: the component id or -1; slice_first [z + 1] int32:
+ * slice s owns ids slice_first[s] .. slice_first[s + 1] - 1; stats [stats_cap, 3] int64: (pixel count, sum of rows, sum of columns) per id,
+ * rows past slice_first[z] unwritten.  stats_cap >= mdt_petct_body_components_capacity(z, y, x) = z * ceil(y x / 2), else MDT_EINVAL;
+ * z y x < 2^31, else MDT_EUNSUPPORTED (both queries return 0 then).  Integer atomics only. */
+long long mdt_petct_body_components_capacity(int z, int y, int x);
+size_t mdt_petct_body_components_workspace_bytes(int z, int y, int x);
+int mdt_petct_body_components(int src_dtype, const void *ct, int z, int y, int x, int *label, int *slice_first, long long *stats, long long stats_cap,
+                              void *ws, size_t ws_bytes, void *stream);
+/* mdt_petct_zcrop_criterion: flags [z] uint8 = 1 where the slice has at least n_comps components of mdt_petct_body_components with count >
+ * min_pix and (rows / count - y / 2)^2 + (cols / count - x / 2)^2 < rad_crit, each operation rounded separately in fp64.  No workspace. */
+int mdt_petct_zcrop_criterion(const int *slice_first, const long long *stats, int z, int y, int x, long long min_pix, int n_comps, double rad_crit,
+                              unsigned char *flags, void *stream);
+/* mdt_petct_normalize: out [2, n] fp32 from the cropped CT ct [n] int16 and PET pet [n] fp32.  CT: c = (1200 + clip(x, -1200, 600)) / 1800,
+ * its mean and population std in fp64, out[0] = fl32((c - mean) / std) in fp64.  PET: mean and population std in fp64, each rounded to fp32,
+ * out[1] = fl32(fl32(p - mean) / std).  stats [4] fp64 (device) = {CT mean, CT std, PET mean, PET std} before rounding.  The sums run over
+ * fixed 1024-way partial sums and fixed trees.  Workspace: 16 KiB. */
+size_t mdt_petct_normalize_workspace_bytes(long long n);
+int mdt_petct_normalize(const short *ct, const float *pet, long long n, float *out, double *stats, void *ws, size_t ws_bytes, void *stream);
+
 /* ------------------------------------------------------------- toy experiment images (csrc/toys.cu) ----------------------------------------
  * replaces: multi_processing_create_image of experiments/toy_exp/generate_toys.py, with a per-image seed in place of numpy's global state.
  *

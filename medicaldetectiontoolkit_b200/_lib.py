@@ -18,6 +18,11 @@ class MdtError(RuntimeError):
     pass
 
 
+class PetctGrid(ctypes.Structure):
+    """mirror of struct mdt_petct_grid (include/mdt_b200.h): an ITK image geometry in (x, y, z) order"""
+    _fields_ = [("size", ctypes.c_int * 3), ("origin", ctypes.c_double * 3), ("spacing", ctypes.c_double * 3), ("direction", ctypes.c_double * 9)]
+
+
 class Conv3dDesc(ctypes.Structure):
     """mirror of struct mdt_conv3d_desc (include/mdt_b200.h)"""
     _fields_ = [(n, ctypes.c_int) for n in (
@@ -120,6 +125,14 @@ SIGNATURES = {
     "mdt_pp_vote_add": (_I, [_VP, _VP, _I64, _I, _VP]),
     "mdt_pp_vote_label": (_I, [_VP, _I64, _I, _I, _VP, _VP, _VP]),
     "mdt_pp_label_summary": (_I, [_VP, _I, _I64, _VP, _VP, _VP]),
+    "mdt_petct_resample": (_I, [_I, _VP, ctypes.POINTER(PetctGrid), _I, _VP, ctypes.POINTER(PetctGrid), _VP]),
+    "mdt_petct_seg_merge": (_I, [_I, _VP, _I, _I, _I, _I, c_i64p, ctypes.POINTER(ctypes.c_ubyte), _VP, _VP]),
+    "mdt_petct_body_components_capacity": (_I64, [_I, _I, _I]),
+    "mdt_petct_body_components_workspace_bytes": (_SZ, [_I, _I, _I]),
+    "mdt_petct_body_components": (_I, [_I, _VP, _I, _I, _I, _VP, _VP, _VP, _I64, _VP, _SZ, _VP]),
+    "mdt_petct_zcrop_criterion": (_I, [_VP, _VP, _I, _I, _I, _I64, _I, _D, _VP, _VP]),
+    "mdt_petct_normalize_workspace_bytes": (_SZ, [_I64]),
+    "mdt_petct_normalize": (_I, [_VP, _VP, _I64, _VP, _VP, _VP, _SZ, _VP]),
     "mdt_toy_images": (_I, [_VP, _I, _I, _I, _I, _I, _VP, _VP, _VP]),
 }
 

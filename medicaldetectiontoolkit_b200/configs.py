@@ -208,6 +208,9 @@ def make_cf(model='retina_unet', dim=3, patch_size=None, exp='lidc_exp', batch_s
     cf.n_workers = 8
     if exp == 'toy_exp':
         cf.n_train_val_data = 1500
+    if exp == PETCT:
+        # petct_preprocessing.py (experiments/pet_ct_tnm_classification/configs.py); the raw and output paths are the user's to set
+        cf.root_dir = cf.raw_data_dir = cf.pp_dir = None
     if exp == 'lidc_exp':
         # preprocessing.py (experiments/lidc_exp/configs.py:31-34); the raw and output paths are the user's to set
         cf.root_dir = cf.raw_data_dir = cf.pp_dir = None

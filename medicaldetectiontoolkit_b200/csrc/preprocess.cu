@@ -4,13 +4,15 @@
 #include <cuda_fp16.h>
 #include <math.h>
 
-#include "mdt_common.cuh"
+#include "pp_reduce.cuh"
 
 namespace {
 
+using mdt::block_tree_sum;
+using mdt::kRedBlocks;
+using mdt::kRedThreads;
+
 constexpr int kMaxRadius = 64;        // gaussian radius int(4 sigma + 0.5) up to a downsampling factor of about 33
-constexpr int kRedBlocks = 1024;      // normalisation: fixed number of partial sums, whatever the device
-constexpr int kRedThreads = 256;
 constexpr double kSigmaMin = 1e-15;   // scipy.ndimage.gaussian_filter skips axes with sigma <= 1e-15
 
 struct GaussW {
@@ -181,16 +183,6 @@ int resample_launch(const void *src, const int in[3], const int outs[3], const R
 bool shape_ok(const int *s) { return s != nullptr && s[0] > 0 && s[1] > 0 && s[2] > 0; }
 
 // ------------------------------------------------------------------------------------------------------------------- normalisation
-__device__ __forceinline__ double block_tree_sum(double v, double *sh) {
-    sh[threadIdx.x] = v;
-    __syncthreads();
-    for (int h = blockDim.x / 2; h > 0; h >>= 1) {
-        if (threadIdx.x < h) sh[threadIdx.x] = __dadd_rn(sh[threadIdx.x], sh[threadIdx.x + h]);
-        __syncthreads();
-    }
-    return sh[0];
-}
-
 // block b covers [b chunk, (b + 1) chunk); thread t sums its elements t, t + 256, ... sequentially.  pass 0: clip x in place and sum x;
 // pass 1: sum (x - mean)^2 with mean = stats[0]
 __global__ void __launch_bounds__(kRedThreads) norm_partial_kernel(float *__restrict__ x, long long n, long long chunk, int pass,
@@ -212,13 +204,6 @@ __global__ void __launch_bounds__(kRedThreads) norm_partial_kernel(float *__rest
     }
     const double s = block_tree_sum(acc, sh);
     if (threadIdx.x == 0) partial[blockIdx.x] = s;
-}
-
-// one block of kRedBlocks threads: the tree over the partial sums.  pass 0: stats[0] = mean; pass 1: stats[1] = population std
-__global__ void __launch_bounds__(kRedBlocks) norm_final_kernel(const double *__restrict__ partial, long long n, int pass, double *__restrict__ stats) {
-    __shared__ double sh[kRedBlocks];
-    const double s = block_tree_sum(partial[threadIdx.x], sh);
-    if (threadIdx.x == 0) stats[pass] = pass == 0 ? s / (double)n : sqrt(s / (double)n);
 }
 
 // x = fl32(fl32(x - fl32(mean)) / float(fp16(fl32(std))))
@@ -317,7 +302,7 @@ int mdt_pp_normalize(float *x, long long n, double *stats, void *ws, size_t ws_b
     for (int pass = 0; pass < 2; ++pass) {
         norm_partial_kernel<<<kRedBlocks, kRedThreads, 0, s>>>(x, n, chunk, pass, stats, partial);
         if (int rc = mdt::launch_status()) return rc;
-        norm_final_kernel<<<1, kRedBlocks, 0, s>>>(partial, n, pass, stats);
+        mdt::red_final_kernel<<<1, kRedBlocks, 0, s>>>(partial, n, pass, stats);
         if (int rc = mdt::launch_status()) return rc;
     }
     norm_apply_kernel<<<grid_for(n, 256), 256, 0, s>>>(x, n, stats);

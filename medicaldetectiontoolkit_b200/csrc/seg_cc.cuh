@@ -1,5 +1,6 @@
 // Connected-component labelling shared by seg_components.cu (Detection U-Net boxes) and seg_rois.cu (ROIs of a training batch's segmentation).
-// Face connectivity: 6 neighbours in 3D, 4 in 2D (scipy's generate_binary_structure(dim, 1)); no neighbour test crosses an element boundary.
+// Face connectivity: 6 neighbours in 3D, 4 in 2D (scipy's generate_binary_structure(dim, 1)), and on request 8 in 2D (petct_preprocess.cu);
+// no neighbour test crosses an element boundary.
 // Every foreground voxel starts as its own union-find root (P[t] = t, background P[t] = -1).  Roots are hooked larger-under-smaller with
 // atomicMin, so every tree's root is the minimum linear index of its component, whatever order the unions ran in; an exclusive scan of the
 // root flags then numbers the components in scipy.ndimage.label's order (by first voxel in C order).  Integer atomics only: deterministic.
@@ -39,8 +40,9 @@ __device__ __forceinline__ void uf_union(int *P, int a, int b) {
     }
 }
 
-// union of every voxel t with label(t) != 0 with each lower (y, x, z) neighbour of the same label
-template <typename Label>
+// union of every voxel t with label(t) != 0 with each lower (y, x, z) neighbour of the same label.  kDiag2D (2D elements, g.Z == 1) also
+// joins the two diagonal neighbours of the row above: 8-connectivity (generate_binary_structure(2, 2))
+template <typename Label, bool kDiag2D = false>
 __global__ void __launch_bounds__(256) cc_merge_kernel(CcGeom g, int *P, Label label) {
     const long long XZ = (long long)g.X * g.Z;
     for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < g.N; t += (long long)gridDim.x * blockDim.x) {
@@ -51,6 +53,10 @@ __global__ void __launch_bounds__(256) cc_merge_kernel(CcGeom g, int *P, Label l
         if (z > 0 && label(t - 1) == c) uf_union(P, (int)t, (int)(t - 1));
         if (x > 0 && label(t - g.Z) == c) uf_union(P, (int)t, (int)(t - g.Z));
         if (y > 0 && label(t - XZ) == c) uf_union(P, (int)t, (int)(t - XZ));
+        if (kDiag2D && y > 0) {
+            if (x > 0 && label(t - XZ - 1) == c) uf_union(P, (int)t, (int)(t - XZ - 1));
+            if (x < g.X - 1 && label(t - XZ + 1) == c) uf_union(P, (int)t, (int)(t - XZ + 1));
+        }
     }
 }
 

@@ -12,7 +12,7 @@ context channels are one batched gather (mdt_loader_gather) from the in-bounds w
 into a pinned staging buffer.  'data' and 'seg' of a training batch are CUDA tensors in the reference's dtypes.
 
 Test batches: PatientBatchIterator uploads each patient once, edge-pads and tiles it into patches with one gather per output, and converts
-the segs to boxes with augment.seg_to_boxes; its batches are host numpy arrays in the reference's format (Predictor.predict_test_set takes
+the segs to boxes with augment.seg_to_boxes (pet_ct_tnm_classification: their connected components with augment.seg_rois); its batches are host numpy arrays in the reference's format (Predictor.predict_test_set takes
 them unchanged).  The box conversion gives 'bb_target', 'roi_labels' and the relabelled 'seg' (no 'roi_masks': the predictor does not read
 them).
 
@@ -254,6 +254,15 @@ class CudaOps(object):
             L.check(L.load().mdt_loader_gather(SRC_DTYPE[dt], L.ptr(src), ptr(0), n, C, I, J, K, ptr(offs[0]), ptr(offs[1]), ptr(offs[2]), ptr(offs[3]),
                                                SRC_DTYPE[np.dtype(out_dtype)], L.ptr(out), L.stream_ptr()))
             return out
+
+    def seg_rois(self, seg, class_target, class_specific):
+        """seg [B, 1, *P] device uint8, class_target [B] host int32 -> (elem_first [B + 1] host int32, stats [elem_first[B], 7] host int32,
+        relabelled seg on the device) of augment.seg_rois"""
+        with torch.cuda.device(self.device):
+            ct = torch.from_numpy(np.ascontiguousarray(class_target, dtype=np.int32)).to(self.device)
+            _, first, stats, seg_out = A.seg_rois(seg.contiguous(), ct, class_specific)
+            first = first.cpu().numpy()
+            return first, stats[:int(first[-1])].cpu().numpy(), seg_out
 
     def seg_to_boxes(self, seg, lut):
         """seg [B, 1, *P] device uint8, lut [B, 256] host uint8 -> (stats [B, 255, 7] host int32, relabelled seg on the device)"""
@@ -522,16 +531,20 @@ def _edge(S, new):
 
 
 class PatientBatchIterator(object):
-    """one patient per batch, as the experiment's PatientBatchIterator.generate_train_batch builds it (lidc_exp and toy_exp): the patient
-    edge-padded to at least cf.patch_size, its patient-level targets (3D, or per slice in 2D plus the 3D targets with merge_2D_to_3D_preds),
-    and, when it is larger than a patch, all its overlapping patches ('patch_crop_coords').  Host numpy arrays in the reference's format."""
+    """one patient per batch, as the experiment's PatientBatchIterator.generate_train_batch builds it: the patient edge-padded to at least
+    cf.patch_size, its patient-level targets (3D, or per slice in 2D plus the 3D targets with merge_2D_to_3D_preds), and, when it is larger
+    than a patch, all its overlapping patches ('patch_crop_coords').  Host numpy arrays in the reference's format.
+
+    pet_ct_tnm_classification: the reference's iterator cannot run (it indexes a file listing with an integer, reads an unset dataset_pids
+    and converts boxes without a seg) and preprocesses raw scans on the fly.  Here it is the lidc_exp iterator on the preprocessed two-channel
+    directory (petct_preprocessing): both image channels (with n_3D_context, the CT's context slices, as BatchGenerator stacks them), the
+    ROIs of the patient and of every patch taken as the connected components of the seg, and the patient's target 0 if its seg has any
+    foreground, else -1 (the rule of the experiment's BatchGenerator)."""
 
     def __init__(self, data, cf, ops=None):
         self._data = data
         self.cf = cf
         self.exp = getattr(cf, 'experiment', 'lidc_exp')
-        if self.exp == PETCT:
-            raise NotImplementedError("pet_ct_tnm_classification's PatientBatchIterator preprocesses raw scans; it is not provided")
         self.ops = ops if ops is not None else CudaOps()
         self.patient_ix = 0
         self.dataset_pids = [v['pid'] for (k, v) in data.items()]
@@ -544,6 +557,10 @@ class PatientBatchIterator(object):
         return self.generate_train_batch()
 
     def _boxes(self, seg, class_targets, dim):
+        if self.exp == PETCT:
+            first, stats, seg_out = self.ops.seg_rois(seg, np.asarray(class_targets, dtype=np.int32).reshape(-1), self.cf.class_specific_seg_flag)
+            bb, labels, _ = A.boxes_from_rois(first, stats, class_targets, dim)
+            return as_array(bb), as_array(labels), self.ops.to_host(seg_out)
         lut = A.label_lut(class_targets, self.cf.class_specific_seg_flag)
         stats, seg_out = self.ops.seg_to_boxes(seg, lut)
         bb, labels, _ = A.boxes_from_stats(stats, class_targets, dim)
@@ -577,19 +594,25 @@ class PatientBatchIterator(object):
         cf = self.cf
         img = np.load(patient['data'], mmap_mode='r')
         seg_f = np.load(patient['seg'], mmap_mode='r')
-        Z, Y, X = img.shape
+        if img.ndim == 3:
+            img = img[None]
+        C, Z, Y, X = img.shape
+        if self.exp == PETCT:
+            targets = np.array([0 if np.asarray(seg_f).any() else -1])
         img_dev = self.ops.upload(img)
         seg_dev = self.ops.upload(seg_f)
-        d_img, d_seg = _src_desc([(1, Z, Y, X)]), _src_desc([(1, Z, Y, X)])
+        d_img, d_seg = _src_desc([(C, Z, Y, X)]), _src_desc([(1, Z, Y, X)])
         P = self.patch_size
         shape = [max(s, p) for s, p in zip((Y, X, Z), P)]
         ey, ex, ez = _edge(Y, shape[0]), _edge(X, shape[1]), _edge(Z, shape[2])
         n3 = cf.n_3D_context
         i32 = lambda a: np.ascontiguousarray(a, dtype=np.int32)
 
-        def gather(src, desc, n, tz, ty, tx, dtype, C=1):
+        def gather(src, desc, n, tz, ty, tx, dtype, chans=(0,)):
+            """chans: the source channel of each output channel; tz [n or 1, C or 1, K] broadcast over them"""
             d = np.repeat(desc, n)
-            tabs = (np.zeros((n, C), np.int32), i32(tz), i32(ty), i32(tx))
+            tz = np.asarray(tz)
+            tabs = (i32(np.tile(chans, (n, 1))), i32(np.broadcast_to(tz, (n, len(chans), tz.shape[-1]))), i32(ty), i32(tx))
             return self.ops.gather(src, d, tabs, dtype, key='test')
 
         def slice_z(zs, context):
@@ -600,6 +623,8 @@ class PatientBatchIterator(object):
             zz = zs[:, None] + np.arange(-n3, n3 + 1)[None]
             return np.where((zz >= 0) & (zz < Z), zz, -1)[..., None]
 
+        chans = np.arange(C)                                   # image channels, or the CT's context slices in 2D with n_3D_context
+        chans2 = np.zeros(2 * n3 + 1, np.int64) if n3 is not None else chans
         patched = any(shape[d] > P[d] for d in range(3))
         out = {}
         if cf.dim == 3 or cf.merge_2D_to_3D_preds:
@@ -609,12 +634,12 @@ class PatientBatchIterator(object):
             if cf.dim == 3:
                 out = {'seg': seg3_out, 'class_target': targets, 'pid': pid, 'bb_target': bb3, 'roi_labels': lab3}
                 if not patched:
-                    out['data'] = self.ops.to_host(gather(img_dev, d_img, 1, ez[None, None], ey[None], ex[None], img.dtype))
+                    out['data'] = self.ops.to_host(gather(img_dev, d_img, 1, ez[None, None], ey[None], ex[None], img.dtype, chans))
             out.update({'patient_bb_target': bb3, 'patient_roi_labels': lab3, 'original_img_shape': shape3})
         if cf.dim == 2:
             Zp = shape[2]
             zs = ez
-            C2 = 2 * n3 + 1 if n3 is not None else 1
+            C2 = len(chans2)
             seg2 = gather(seg_dev, d_seg, Zp, slice_z(zs, False), np.tile(ey, (Zp, 1)), np.tile(ex, (Zp, 1)), np.uint8)[..., 0]
             targets2 = np.array(np.repeat(targets, Zp, axis=0))
             bb2, lab2, seg2_out = self._boxes(seg2, targets2, 2)
@@ -622,7 +647,7 @@ class PatientBatchIterator(object):
             out_2d = {'seg': seg2_out, 'class_target': targets2, 'pid': pid, 'bb_target': bb2, 'roi_labels': lab2, 'original_img_shape': shape2}
             if not patched:
                 out_2d['data'] = self.ops.to_host(gather(img_dev, d_img, Zp, slice_z(zs, n3 is not None), np.tile(ey, (Zp, 1)), np.tile(ex, (Zp, 1)),
-                                                         img.dtype, C=C2)[..., 0])
+                                                         img.dtype, chans2)[..., 0])
             if cf.merge_2D_to_3D_preds:
                 out_2d.update({'patient_bb_target': out['patient_bb_target'], 'patient_roi_labels': out['patient_roi_labels']})
             else:
@@ -636,12 +661,11 @@ class PatientBatchIterator(object):
         tx = np.stack([ex[c[2]:c[3]] for c in coords])
         if cf.dim == 3:
             tz = np.stack([ez[c[4]:c[5]] for c in coords])[:, None]
-            data = gather(img_dev, d_img, n, tz, ty, tx, img.dtype)
+            data = gather(img_dev, d_img, n, tz, ty, tx, img.dtype, chans)
             seg = gather(seg_dev, d_seg, n, tz, ty, tx, np.uint8)
         else:
             zs = ez[coords[:, 4]]
-            C2 = 2 * n3 + 1 if n3 is not None else 1
-            data = gather(img_dev, d_img, n, slice_z(zs, n3 is not None), ty, tx, img.dtype, C=C2)[..., 0]
+            data = gather(img_dev, d_img, n, slice_z(zs, n3 is not None), ty, tx, img.dtype, chans2)[..., 0]
             seg = gather(seg_dev, d_seg, n, slice_z(zs, False), ty, tx, np.uint8)[..., 0]
         targets_p = np.repeat(targets, n, axis=0)
         bb, labels, seg_out = self._boxes(seg, targets_p, cf.dim)
