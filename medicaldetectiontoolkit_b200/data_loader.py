@@ -737,10 +737,22 @@ def get_train_generators(cf, logger):
     return batch_gen
 
 
-def get_test_generator(cf, logger):
+def get_test_generator(cf, logger, rank=None, world_size=None):
     """{'test': PatientBatchIterator, 'n_test'}: the hold-out directory cf.pp_test_data_path with cf.hold_out_test_set, else the fold's test
-    split of cf.exp_dir's fold pickle"""
+    split of cf.exp_dir's fold pickle.
+
+    With rank and world_size (one process per GPU): the first n_test patients (the cf.max_test_patients cap on the whole ordered list) are
+    sharded round-robin, and this rank keeps positions rank, rank + world_size, ...  Its iterator reads only those patients, 'n_test' is
+    their count (0 when world_size exceeds it), and 'shard_positions' (their positions in the capped list) and 'world_size' make
+    Predictor.predict_test_set gather every rank's results to rank 0."""
+    import operator
     import pickle
+    if (rank is None) != (world_size is None):
+        raise ValueError("get_test_generator: give both rank and world_size or neither (rank={}, world_size={})".format(rank, world_size))
+    if world_size is not None:
+        rank, world_size = operator.index(rank), operator.index(world_size)
+        if not 0 <= rank < world_size:
+            raise ValueError("get_test_generator: rank {} is outside [0, world_size = {})".format(rank, world_size))
     if cf.hold_out_test_set:
         test_ix = None
     else:
@@ -749,4 +761,11 @@ def get_test_generator(cf, logger):
     test_data = load_dataset(cf, logger, test_ix, pp_data_path=cf.pp_test_data_path)
     n = len(test_data)
     logger.info("data set loaded with: {} test patients".format(n))
-    return {'test': PatientBatchIterator(test_data, cf), 'n_test': n if cf.max_test_patients == "all" else min(cf.max_test_patients, n)}
+    n_test = n if cf.max_test_patients == "all" else min(cf.max_test_patients, n)
+    if world_size is None:
+        return {'test': PatientBatchIterator(test_data, cf), 'n_test': n_test}
+    positions = list(range(rank, n_test, world_size))
+    patients = list(test_data.items())
+    logger.info("rank {} of {}: {} of the {} test patients".format(rank, world_size, len(positions), n_test))
+    return {'test': PatientBatchIterator(OrderedDict(patients[p] for p in positions), cf), 'n_test': len(positions),
+            'shard_positions': positions, 'world_size': world_size}

@@ -8,6 +8,10 @@
 Same arguments (numpy arrays / lists of box dicts) and return values as the reference, so `Predictor` can call them unchanged; the greedy cluster
 loops run in one kernel each on the current CUDA device (fp64, the reference's expression order).  No CPU fallback.
 """
+import io
+import pickle
+import sys
+
 import numpy as np
 import torch
 
@@ -123,6 +127,36 @@ def get_mirrored_patch_crops(patch_crops, org_img_shape):
     return [[flip_y(c) for c in patch_crops], [flip_x(c) for c in patch_crops], [flip_x(flip_y(c)) for c in patch_crops]]
 
 
+class _SharedPickler(pickle.Pickler):
+    """Pickles one rank's predictions for the gather to rank 0.  pickle writes an object once per identity, so rank 0's raw_pred_boxes file
+    has the bytes of a single-process run only if the merged lists share objects across patients as that run's do: interned strings
+    (dict keys, 'det', 'gt') and numpy's built-in dtypes.  Those go by value and _SharedUnpickler resolves them to rank 0's own objects."""
+
+    def persistent_id(self, obj):
+        # sys.intern of a fresh equal string returns the interned copy if there is one (else it interns the fresh string, not obj)
+        if type(obj) is str and sys.intern((obj + ' ')[:-1]) is obj:
+            return b's' + obj.encode('utf-8', 'surrogatepass')
+        if isinstance(obj, np.dtype) and np.dtype(obj.str) is obj:
+            return b'd' + obj.str.encode()
+        return None
+
+
+class _SharedUnpickler(pickle.Unpickler):
+    def persistent_load(self, pid):
+        value = pid[1:].decode('utf-8', 'surrogatepass')
+        return sys.intern(value) if pid[:1] == b's' else np.dtype(value)
+
+
+def _dumps_shared(obj):
+    buf = io.BytesIO()
+    _SharedPickler(buf).dump(obj)
+    return buf.getvalue()
+
+
+def _loads_shared(data):
+    return _SharedUnpickler(io.BytesIO(data)).load()
+
+
 class Predictor:
     """Patient-level prediction pipeline with the call surface of the reference's `Predictor` (predictor.py:27-284): patches are forwarded in chunks of
     `cf.batch_size` (`batch_tiling_forward`), box and segmentation outputs are moved back to patient coordinates (`spatial_tiling_forward`), test
@@ -165,16 +199,72 @@ class Predictor:
                 results_dict['boxes'] = merge_2D_to_3D_preds_per_patient([results_dict['boxes'], 'dummy_pid', self.cf.class_dict, self.cf.merge_3D_iou])[0]
         return results_dict
 
+    def _net_device(self):
+        try:
+            return next(iter(self.net.parameters())).device
+        except (StopIteration, AttributeError, TypeError):
+            return torch.device('cpu')
+
     # -- predictor.py:122-211
     def predict_test_set(self, batch_gen, return_results=True):
+        """Temporal ensemble over the ranked checkpoints, mirrored passes with cf.test_aug; writes raw_pred_boxes_list.pickle (with
+        cf.hold_out_test_set raw_pred_boxes_hold_out_list.pickle) to cf.fold_dir and returns the consolidated per-patient results.
+
+        A generator from get_test_generator(cf, logger, rank, world_size) holds one rank's shard of the test set: every rank of the default
+        process group (whose size must be the generator's world_size) predicts and consolidates its own patients, and rank 0 gathers them,
+        writes the file in the global patient order and returns the results; the other ranks write nothing and return None.  The file's
+        bytes and the results do not depend on the world size."""
+        if 'world_size' in batch_gen:
+            return self._predict_test_shard(batch_gen, return_results)
+        out = self._predict_raw(batch_gen)
+        self._write_raw(out)
+        if return_results:
+            return self._consolidate(out, self.n_ens, apply_wbc=True)
+
+    def _predict_test_shard(self, batch_gen, return_results):
+        import torch.distributed as dist
+        world = batch_gen['world_size']
+        if not (dist.is_available() and dist.is_initialized()):
+            raise RuntimeError('predict_test_set: the test generator is sharded over {} ranks, but no process group is initialised'.format(world))
+        if dist.get_world_size() != world:
+            raise RuntimeError('predict_test_set: the test generator is sharded over {} ranks, but the process group has {}'.format(
+                world, dist.get_world_size()))
+        out = self._predict_raw(batch_gen)
+        results = self._consolidate(out, self.n_ens, apply_wbc=True) if return_results else None
+        rank = dist.get_rank()
+        gathered = [None] * world if rank == 0 else None
+        dist.gather_object(None if rank == 0 else _dumps_shared((batch_gen['shard_positions'], out, results)), gathered, dst=0)
+        if rank != 0:
+            return None
+        parts = [(batch_gen['shard_positions'], out, results)] + [_loads_shared(b) for b in gathered[1:]]
+        n = sum(len(p[0]) for p in parts)
+        raw_all, results_all = [None] * n, [None] * n
+        for positions, raw, res in parts:
+            for j, pos in enumerate(positions):
+                if not 0 <= pos < n or raw_all[pos] is not None:
+                    raise RuntimeError('predict_test_set: the ranks\' shards do not partition the test set (position {} of {})'.format(pos, n))
+                raw_all[pos] = raw[j]
+                if return_results:
+                    results_all[pos] = res[j]
+        self._write_raw(raw_all)
+        if return_results:
+            return results_all
+
+    def _write_raw(self, out):
         import os
-        import pickle
+        name = 'raw_pred_boxes_hold_out_list' if self.cf.hold_out_test_set else 'raw_pred_boxes_list'
+        with open(os.path.join(self.cf.fold_dir, '{}.pickle'.format(name)), 'wb') as handle:
+            pickle.dump(out, handle)
+
+    def _predict_raw(self, batch_gen):
+        """[[boxes per batch element (every ensemble member's detections, then the GT boxes), pid] per patient] in batch_gen's order"""
+        import os
         from collections import OrderedDict
         patients = OrderedDict()
         for rank_ix, epoch in enumerate(self.epoch_ranking):
             weight_path = os.path.join(self.cf.fold_dir, '{}_best_checkpoint'.format(epoch), 'params.pth')
             self._info('tmp ensembling over rank_ix:{} epoch:{}'.format(rank_ix, weight_path))
-            self.net.load_state_dict(torch.load(weight_path))
+            self.net.load_state_dict(torch.load(weight_path, map_location=self._net_device()))
             self.net.eval()
             self.rank_ix = str(rank_ix)
             with torch.no_grad():
@@ -193,11 +283,7 @@ class Predictor:
                 for t in range(len(p['patient_bb_target'][b])):
                     boxes[b].append({'box_coords': p['patient_bb_target'][b][t], 'box_label': p['patient_roi_labels'][b][t], 'box_type': 'gt'})
             out.append([boxes, pid])
-        name = 'raw_pred_boxes_hold_out_list' if self.cf.hold_out_test_set else 'raw_pred_boxes_list'
-        with open(os.path.join(self.cf.fold_dir, '{}.pickle'.format(name)), 'wb') as handle:
-            pickle.dump(out, handle)
-        if return_results:
-            return self._consolidate(out, self.n_ens, apply_wbc=True)
+        return out
 
     # -- predictor.py:214-284
     def load_saved_predictions(self, apply_wbc=False):
@@ -278,10 +364,7 @@ class Predictor:
         patches = self.batch_tiling_forward(batch)
         shp = tuple(batch['original_img_shape'])
         results_dict = {'boxes': [[] for _ in range(shp[0])]}
-        try:
-            dev = next(iter(self.net.parameters())).device
-        except (StopIteration, AttributeError, TypeError):
-            dev = torch.device('cpu')
+        dev = self._net_device()
         # segmentation: sum of the patch label maps in float16 + overlap counts, then the mean where at least one patch contributes
         seg = torch.zeros((shp[0], 1) + shp[2:], dtype=torch.float16, device=dev)
         cnt = torch.zeros_like(seg, dtype=torch.uint8)
