@@ -218,6 +218,30 @@ int mdt_seg_loss_weighted_forward(const float *logits, const long long *strides3
 int mdt_seg_loss_weighted_backward(const float *logits, const long long *strides3, const unsigned char *target, int n, long long voxels, int n_classes,
                                    float false_positive_weight, float smooth, const float *class_weights, const double *sums, const float *grad_out2,
                                    float *grad_logits, void *stream);
+/* The seg loss of a batch split across ranks.  mdt_seg_loss_sample_sums (+ _weighted): rows (device, [n][3*n_classes + 1] doubles) = the sums
+ * layout above for each sample alone; the grid is (sample, chunk) with a chunk count that depends on (voxels, n_classes) only and every sum is
+ * fp64 in a fixed order, so a sample's row is bit-identical in a batch of any size.  Workspace: mdt_seg_loss_sample_workspace_bytes (0 =
+ * unsupported arguments).  mdt_seg_loss_from_sums: rows [n_total][3*n_classes + 1] (all ranks' rows, rank-major) added in row order -> sums and
+ * out2 as mdt_seg_loss_forward; the unweighted CE denominator is n_total * voxels, the weighted one sum_c w[c] tsum_c (class_weights NULL =
+ * unweighted).  mdt_seg_loss_backward_global (+ _weighted): mdt_seg_loss_backward over this rank's n samples with the global sums and the
+ * unweighted CE denominator total_voxels (>= n * voxels); grad_out2 holds n_ranks >= 1 pairs {dL/d dice_score, dL/d ce} (every rank's, in
+ * rank order), added in fp64 in that order.
+ * mdt_exchange_fill: count elements of buf set to -0.0 (f64 = 1: doubles, 0: floats), the fill of an exchange buffer whose slots each rank
+ * writes before an all_reduce(SUM): v + (-0.0) = v for every v, so every slot arrives with its bits. */
+size_t mdt_seg_loss_sample_workspace_bytes(int n, long long voxels, int n_classes);
+int mdt_seg_loss_sample_sums(const float *logits, const long long *strides3, const unsigned char *target, int n, long long voxels, int n_classes,
+                             double *rows, void *ws, size_t ws_bytes, void *stream);
+int mdt_seg_loss_weighted_sample_sums(const float *logits, const long long *strides3, const unsigned char *target, int n, long long voxels,
+                                      int n_classes, const float *class_weights, double *rows, void *ws, size_t ws_bytes, void *stream);
+int mdt_seg_loss_from_sums(const double *rows, int n_total, long long voxels, int n_classes, float false_positive_weight, float smooth,
+                           const float *class_weights, double *sums, float *out2, void *stream);
+int mdt_seg_loss_backward_global(const float *logits, const long long *strides3, const unsigned char *target, int n, long long voxels, int n_classes,
+                                 float false_positive_weight, float smooth, const double *sums, long long total_voxels, const float *grad_out2,
+                                 int n_ranks, float *grad_logits, void *stream);
+int mdt_seg_loss_weighted_backward_global(const float *logits, const long long *strides3, const unsigned char *target, int n, long long voxels,
+                                          int n_classes, float false_positive_weight, float smooth, const float *class_weights, const double *sums,
+                                          long long total_voxels, const float *grad_out2, int n_ranks, float *grad_logits, void *stream);
+int mdt_exchange_fill(void *buf, long long count, int f64, void *stream);
 
 /* ------------------------------------------------------------- segmentation connected components (csrc/seg_components.cu) ------------------
  * replaces: softmax + D2H copy + per-class argmax mask + get_coords (scipy.ndimage.label, np.unique, argsort, one full-volume mask per kept
@@ -289,6 +313,23 @@ int mdt_norm_apply(const float *x, const float *mean, const float *rstd, const f
 int mdt_norm_backward(const float *dy, const float *y, const float *x, const float *mean, const float *rstd, const float *gamma, int n, long long s,
                       int c, int per_sample, int act, float slope, int batch_stats, float *dx, float *dgamma, float *dbeta, float *dresidual, void *ws,
                       size_t ws_bytes, void *stream);
+/* Batch norm over a batch split across ranks (per_sample = 0 semantics, x [n, s, c] as above).  mdt_norm_sample_sums: sums (device, [n][c]
+ * double pairs (sum x, sum x^2), 16-byte aligned) of each sample; a sample's row split depends on (s, c) only, so its sums are bit-identical in a
+ * batch of any size.  mdt_norm_stats_from_sums: rows [n_total][c] (all ranks' rows, rank-major) added in row order -> mean / rstd over
+ * M = n_total * s, and the running statistics (unbiased with that M; n_total * s >= 2) and num_batches_tracked as mdt_norm_stats.
+ * mdt_norm_backward_sample_sums: per-sample (sum g, sum g xhat) with g = dy * act'(y), as mdt_norm_backward.  mdt_norm_backward_from_sums: dx
+ * with the totals of global_sums [n_total][c] and M = n_total * s; dgamma / dbeta = the sums of this rank's rows [local_first_row,
+ * local_first_row + n) in order; dresidual = g.  Workspace (every sample-sum entry point and the from-sums backward):
+ * mdt_norm_sample_workspace_bytes, 0 = unsupported arguments. */
+size_t mdt_norm_sample_workspace_bytes(int n, long long s, int c);
+int mdt_norm_sample_sums(const float *x, int n, long long s, int c, double *sums, void *ws, size_t ws_bytes, void *stream);
+int mdt_norm_stats_from_sums(const double *sums, int n_total, long long s, int c, float eps, float momentum, float *mean, float *rstd,
+                             float *running_mean, float *running_var, long long *num_batches_tracked, void *stream);
+int mdt_norm_backward_sample_sums(const float *dy, const float *y, const float *x, const float *mean, const float *rstd, int n, long long s, int c,
+                                  int act, float slope, double *sums, void *ws, size_t ws_bytes, void *stream);
+int mdt_norm_backward_from_sums(const float *dy, const float *y, const float *x, const float *mean, const float *rstd, const float *gamma,
+                                const double *global_sums, int n_total, int local_first_row, int n, long long s, int c, int act, float slope, float *dx,
+                                float *dgamma, float *dbeta, float *dresidual, void *ws, size_t ws_bytes, void *stream);
 int mdt_act_forward(const float *x, long long count, int act, float slope, float *y, void *stream);
 int mdt_act_backward(const float *dy, const float *y, long long count, int act, float slope, float *dx, void *stream);
 

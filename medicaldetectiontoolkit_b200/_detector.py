@@ -65,6 +65,13 @@ class Detector(nn.Module):
             t = t.pin_memory()
         return t.to(dev, non_blocking=True).to(dtype)
 
+    # the process group of parallel.sync_batch_statistics (None: every statistic is per rank)
+    sync_group = None
+
+    def seg_loss_group(self):
+        """the group the seg loss is taken over: sync_group in training mode, None (per rank) in eval mode"""
+        return self.sync_group if self.training else None
+
     def _seg_to_device(self, seg, fused_losses):
         """label map (b, 1, y, x, (z)) -> device: uint8 (1 byte per voxel over PCIe) for the fused seg loss, int64 for the torch-op one"""
         fused = fused_losses and next(self.parameters()).is_cuda and self.cf.num_seg_classes <= 8
@@ -129,13 +136,15 @@ def anchor_losses(matched, class_logits, pred_deltas, cf, class_loss_fn, bbox_lo
     return class_loss, bbox_loss, monitor
 
 
-def seg_loss_terms(seg_logits, seg, cf):
+def seg_loss_terms(seg_logits, seg, cf, group=None):
     """-> (1 - soft dice, cross-entropy) of the seg logits against the label map (b, 1, y, x, (z)).  uint8 labels (Detector._seg_to_device):
     one pass over the logits and the labels each way in the fused kernel (csrc/loss_ops.cu), no one-hot / probability volumes; int64 labels:
-    the formulation in torch ops."""
+    the formulation in torch ops.  group: take both terms over the batch of all its ranks (fused kernel only)."""
     if seg.dtype == torch.uint8:
-        dice_score, seg_ce = native_ops.seg_loss(seg_logits, seg.contiguous())
+        dice_score, seg_ce = native_ops.seg_loss(seg_logits, seg.contiguous(), group=group)
         return 1 - dice_score, seg_ce
+    if group is not None:
+        raise RuntimeError("seg_loss_terms: the seg loss over a process group runs on the fused kernel only (uint8 labels, <= 8 classes)")
     seg_ohe = F.one_hot(seg[:, 0], cf.num_seg_classes).movedim(-1, 1).float()  # on-device one-hot (reference: numpy)
     return 1 - mutils.batch_dice(F.softmax(seg_logits, dim=1), seg_ohe), F.cross_entropy(seg_logits, seg[:, 0])
 

@@ -84,6 +84,13 @@ SIGNATURES = {
     "mdt_seg_loss_backward": (_I, [_VP, c_i64p, _VP, _I, _I64, _I, _F, _F, _VP, _VP, _VP, _VP]),
     "mdt_seg_loss_weighted_forward": (_I, [_VP, c_i64p, _VP, _I, _I64, _I, _F, _F, _VP, _VP, _VP, _VP, _SZ, _VP]),
     "mdt_seg_loss_weighted_backward": (_I, [_VP, c_i64p, _VP, _I, _I64, _I, _F, _F, _VP, _VP, _VP, _VP, _VP]),
+    "mdt_seg_loss_sample_workspace_bytes": (_SZ, [_I, _I64, _I]),
+    "mdt_seg_loss_sample_sums": (_I, [_VP, c_i64p, _VP, _I, _I64, _I, _VP, _VP, _SZ, _VP]),
+    "mdt_seg_loss_weighted_sample_sums": (_I, [_VP, c_i64p, _VP, _I, _I64, _I, _VP, _VP, _VP, _SZ, _VP]),
+    "mdt_seg_loss_from_sums": (_I, [_VP, _I, _I64, _I, _F, _F, _VP, _VP, _VP, _VP]),
+    "mdt_seg_loss_backward_global": (_I, [_VP, c_i64p, _VP, _I, _I64, _I, _F, _F, _VP, _I64, _VP, _I, _VP, _VP]),
+    "mdt_seg_loss_weighted_backward_global": (_I, [_VP, c_i64p, _VP, _I, _I64, _I, _F, _F, _VP, _VP, _I64, _VP, _I, _VP, _VP]),
+    "mdt_exchange_fill": (_I, [_VP, _I64, _I, _VP]),
     "mdt_seg_components_workspace_bytes": (_SZ, [_I, _I, _I, _I, _I, _I, _I, _I]),
     "mdt_seg_components": (_I, [_VP, c_i64p, _I, _I, _I, _I, _I, _I, _I, _I, _I, _VP, _VP, _VP, _VP, _VP, _VP, _SZ, _VP]),
     "mdt_shem_workspace_bytes": (_SZ, [_I, _I]),
@@ -98,6 +105,11 @@ SIGNATURES = {
     "mdt_norm_eval_stats": (_I, [_VP, _VP, _I, _F, _VP, _VP, _VP]),
     "mdt_norm_apply": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _I, _I64, _I, _I, _I, _F, _VP, _VP]),
     "mdt_norm_backward": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _I, _I64, _I, _I, _I, _F, _I, _VP, _VP, _VP, _VP, _VP, _SZ, _VP]),
+    "mdt_norm_sample_workspace_bytes": (_SZ, [_I, _I64, _I]),
+    "mdt_norm_sample_sums": (_I, [_VP, _I, _I64, _I, _VP, _VP, _SZ, _VP]),
+    "mdt_norm_stats_from_sums": (_I, [_VP, _I, _I64, _I, _F, _F, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "mdt_norm_backward_sample_sums": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I64, _I, _I, _F, _VP, _VP, _SZ, _VP]),
+    "mdt_norm_backward_from_sums": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I64, _I, _I, _F, _VP, _VP, _VP, _VP, _VP, _SZ, _VP]),
     "mdt_act_forward": (_I, [_VP, _I64, _I, _F, _VP, _VP]),
     "mdt_act_backward": (_I, [_VP, _VP, _I64, _I, _F, _VP, _VP]),
     "mdt_augment_gaussian_workspace_bytes": (_SZ, [_I, _I, ctypes.POINTER(_I)]),

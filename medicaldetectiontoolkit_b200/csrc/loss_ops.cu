@@ -153,20 +153,27 @@ __global__ void __launch_bounds__(256) seg_loss_fwd_kernel(const float *__restri
 // d(logits) for  L = g_dice * dice_score + g_ce * ce :
 //   dL/dp_c(v) = g_dice / (C-1) * (2 y_c / D_c - (2 I_c + s) fpw / D_c^2)  (c >= 1),   dL/dz_k = p_k (q_k - sum_c q_c p_c) + g_ce / N (p_k - y_k)
 // (kWeighted: the CE term is g_ce w[y] / sum_c w[c] tsum_c (p_k - y_k))
+// ce_count: the unweighted CE denominator (this launch's n * vox, or the voxel count of the whole batch across ranks)
 template <bool kWeighted>
 __global__ void __launch_bounds__(256) seg_loss_bwd_kernel(const float *__restrict__ logits, const unsigned char *__restrict__ target, SegGeom g, float fpw,
                                                            float smooth, const float *__restrict__ cw, const double *__restrict__ sums,
-                                                           const float *__restrict__ gout, float *__restrict__ grad) {
+                                                           const float *__restrict__ gout, int gout_rows, long long ce_count, float *__restrict__ grad) {
     float qa[kMaxCls], qb[kMaxCls], W[kMaxCls];
     const long long total = (long long)g.n * g.vox;
-    double denom = (double)total;
+    double denom = (double)ce_count;
 #pragma unroll
     for (int c = 0; c < kMaxCls; ++c) W[c] = (kWeighted && c < g.C) ? cw[c] : 1.f;
     if (kWeighted) {
         denom = 0.0;
         for (int c = 0; c < g.C; ++c) denom += (double)cw[c] * sums[2 * g.C + c];
     }
-    const float gd = gout[0], gce = gout[1] / (float)denom;
+    // gout: gout_rows pairs (one per rank) added in row order in fp64 from -0.0 (one row: exactly gout itself)
+    double gsum0 = -0.0, gsum1 = -0.0;
+    for (int r = 0; r < gout_rows; ++r) {
+        gsum0 += (double)gout[2 * r];
+        gsum1 += (double)gout[2 * r + 1];
+    }
+    const float gd = (float)gsum0, gce = (float)gsum1 / (float)denom;
 #pragma unroll
     for (int c = 0; c < kMaxCls; ++c) {
         qa[c] = qb[c] = 0.f;
@@ -211,6 +218,128 @@ __global__ void __launch_bounds__(256) seg_loss_bwd_kernel(const float *__restri
                 const float q = (c == lab ? qa[c] : 0.f) - qb[c];
                 grad[off + c * g.sc] = zz[c] * (q - dot) + (kWeighted ? gce * wl : gce) * (zz[c] - y);
             }
+    }
+}
+
+// ------------------------------------------------------------------------- per-sample seg-loss sums (the batch dice across ranks)
+// rows[b] = the sums layout above for sample b alone.  The grid is (sample, chunk) with a chunk count that depends on (vox, C) only, and every
+// sum is fp64 from the first add in a fixed order (thread: its voxels in order; block: warps in order; chunks: one warp in lane order then a
+// fixed butterfly), so a sample's row has the same bits in a batch of any size.
+constexpr int kSegSampleChunks = 512;        // chunks per sample at most (a batch of one still fills the SMs) ...
+constexpr long long kSegMinChunkVox = 2048;  // ... with at least this many voxels per chunk
+
+__host__ __device__ inline int seg_sample_chunks(long long vox) {
+    const long long c = (vox + kSegMinChunkVox - 1) / kSegMinChunkVox;
+    return (int)(c < kSegSampleChunks ? c : kSegSampleChunks);
+}
+
+template <bool kWeighted>
+__global__ void __launch_bounds__(256) seg_sample_partials_kernel(const float *__restrict__ logits, const unsigned char *__restrict__ target, SegGeom g,
+                                                                  int chunks, const float *__restrict__ cw, double *__restrict__ partial) {
+    double I[kMaxCls], P[kMaxCls], T[kMaxCls];
+    float W[kMaxCls];
+    double ce = 0.0;
+#pragma unroll
+    for (int c = 0; c < kMaxCls; ++c) {
+        I[c] = P[c] = T[c] = 0.0;
+        W[c] = (kWeighted && c < g.C) ? cw[c] : 1.f;
+    }
+    const int b = blockIdx.x / chunks, k = blockIdx.x % chunks;
+    const long long per = (g.vox + chunks - 1) / chunks, v0 = (long long)k * per, v1 = v0 + per < g.vox ? v0 + per : g.vox;
+    for (long long v = v0 + threadIdx.x; v < v1; v += blockDim.x) {
+        const float *z = logits + b * g.sb + v * g.sv;
+        const int lab = target[b * g.vox + v];
+        float zz[kMaxCls];
+        float m = -INFINITY, zt = 0.f;
+#pragma unroll
+        for (int c = 0; c < kMaxCls; ++c)
+            if (c < g.C) {
+                zz[c] = __ldg(z + c * g.sc);
+                m = fmaxf(m, zz[c]);
+                if (c == lab) zt = zz[c];
+            }
+        float s = 0.f;
+#pragma unroll
+        for (int c = 0; c < kMaxCls; ++c)
+            if (c < g.C) { zz[c] = expf(zz[c] - m); s += zz[c]; }
+        const float inv = 1.f / s;
+        const float nlp = logf(s) + (m - zt);   // log-sum-exp form, as in seg_loss_fwd_kernel
+#pragma unroll
+        for (int c = 0; c < kMaxCls; ++c)
+            if (c < g.C) {
+                const float p = zz[c] * inv;
+                P[c] += (double)p;
+                if (c == lab) {
+                    I[c] += (double)p;
+                    T[c] += 1.0;
+                    ce += kWeighted ? (double)(W[c] * nlp) : (double)nlp;
+                }
+            }
+    }
+    __shared__ double s_red[8][3 * kMaxCls + 1];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nv = 3 * g.C + 1;
+#pragma unroll
+    for (int c = 0; c < kMaxCls; ++c)
+        if (c < g.C) {
+            const double a = warp_sum_d(I[c]), p = warp_sum_d(P[c]), d = warp_sum_d(T[c]);
+            if (lane == 0) { s_red[warp][c] = a; s_red[warp][g.C + c] = p; s_red[warp][2 * g.C + c] = d; }
+        }
+    {
+        const double a = warp_sum_d(ce);
+        if (lane == 0) s_red[warp][3 * g.C] = a;
+    }
+    __syncthreads();
+    if ((int)threadIdx.x < nv) {
+        double a = 0.0;
+        for (int w = 0; w < 8; ++w) a += s_red[w][threadIdx.x];
+        partial[(size_t)blockIdx.x * nv + threadIdx.x] = a;
+    }
+}
+
+// one warp per (sample, value): the sample's chunk partials in lane order, then a fixed butterfly
+__global__ void seg_sample_rows_kernel(const double *__restrict__ partial, int n, int chunks, int nv, double *__restrict__ rows) {
+    const long long w = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (w >= (long long)n * nv) return;   // whole warps
+    const int b = (int)(w / nv), j = (int)(w % nv);
+    double a = 0.0;
+    for (int k = lane; k < chunks; k += 32) a += partial[((size_t)b * chunks + k) * nv + j];
+    a = warp_sum_d(a);
+    if (lane == 0) rows[(size_t)b * nv + j] = a;
+}
+
+// rows [N][3C+1] in sample order -> sums (added in order) and out2 = {dice score, cross-entropy}, the finalisation of seg_loss_fwd_kernel
+__global__ void seg_from_sums_kernel(const double *__restrict__ rows, int N, long long vox, int C, float fpw, float smooth, const float *__restrict__ cw,
+                                     double *__restrict__ sums, float *__restrict__ out) {
+    __shared__ double s_sum[3 * kMaxCls + 1];
+    const int nv = 3 * C + 1;
+    if ((int)threadIdx.x < nv) {
+        double a = 0.0;
+        for (int b = 0; b < N; ++b) a += rows[(size_t)b * nv + threadIdx.x];
+        s_sum[threadIdx.x] = a;
+        sums[threadIdx.x] = a;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double dice = 0.0;
+        for (int c = 1; c < C; ++c)
+            dice += (2.0 * s_sum[c] + (double)smooth) / ((double)fpw * s_sum[C + c] + s_sum[2 * C + c] + (double)smooth);
+        out[0] = (float)(C > 1 ? dice / (C - 1) : 0.0);
+        double denom = (double)N * (double)vox;
+        if (cw != nullptr) {
+            denom = 0.0;
+            for (int c = 0; c < C; ++c) denom += (double)cw[c] * s_sum[2 * C + c];
+        }
+        out[1] = (float)(s_sum[3 * C] / denom);
+    }
+}
+
+// -0.0 in every element of an exchange buffer (fp64 or fp32): v + (-0.0) = v for every v, so an all_reduce(SUM) of buffers whose slots only
+// their owner wrote delivers each slot with its bits
+__global__ void __launch_bounds__(256) neg_zero_fill_kernel(void *__restrict__ buf, long long count, int f64) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < count; i += (long long)gridDim.x * blockDim.x) {
+        if (f64) reinterpret_cast<double *>(buf)[i] = -0.0;
+        else reinterpret_cast<float *>(buf)[i] = -0.0f;
     }
 }
 
@@ -470,8 +599,10 @@ static int seg_loss_forward(const float *logits, const long long *strides3, cons
 
 static int seg_loss_backward(const float *logits, const long long *strides3, const unsigned char *target, int n, long long voxels, int n_classes,
                              float false_positive_weight, float smooth, const float *class_weights, const double *sums, const float *grad_out2,
-                             float *grad_logits, void *stream) {
-    if (!logits || !strides3 || !target || !sums || !grad_out2 || !grad_logits || n <= 0 || voxels <= 0) return MDT_EINVAL;
+                             int gout_rows, long long ce_count, float *grad_logits, void *stream) {
+    if (!logits || !strides3 || !target || !sums || !grad_out2 || !grad_logits || n <= 0 || voxels <= 0 || ce_count < (long long)n * voxels ||
+        gout_rows < 1)
+        return MDT_EINVAL;
     if (n_classes < 1 || n_classes > mdt::kMaxCls) return MDT_EUNSUPPORTED;
     mdt::SegGeom g{n, n_classes, voxels, strides3[0], strides3[1], strides3[2]};
     long long blocks = mdt::ceil_div<long long>((long long)n * voxels, 256 * 2);
@@ -479,10 +610,10 @@ static int seg_loss_backward(const float *logits, const long long *strides3, con
     if (blocks < 1) blocks = 1;
     if (class_weights)
         mdt::seg_loss_bwd_kernel<true><<<(unsigned)blocks, 256, 0, mdt::as_stream(stream)>>>(logits, target, g, false_positive_weight, smooth, class_weights,
-                                                                                              sums, grad_out2, grad_logits);
+                                                                                              sums, grad_out2, gout_rows, ce_count, grad_logits);
     else
         mdt::seg_loss_bwd_kernel<false><<<(unsigned)blocks, 256, 0, mdt::as_stream(stream)>>>(logits, target, g, false_positive_weight, smooth, nullptr,
-                                                                                               sums, grad_out2, grad_logits);
+                                                                                               sums, grad_out2, gout_rows, ce_count, grad_logits);
     return mdt::launch_status();
 }
 
@@ -497,8 +628,8 @@ int mdt_seg_loss_forward(const float *logits, const long long *strides3, const u
 
 int mdt_seg_loss_backward(const float *logits, const long long *strides3, const unsigned char *target, int n, long long voxels, int n_classes,
                           float false_positive_weight, float smooth, const double *sums, const float *grad_out2, float *grad_logits, void *stream) {
-    return mdt::seg_loss_backward(logits, strides3, target, n, voxels, n_classes, false_positive_weight, smooth, nullptr, sums, grad_out2, grad_logits,
-                                  stream);
+    return mdt::seg_loss_backward(logits, strides3, target, n, voxels, n_classes, false_positive_weight, smooth, nullptr, sums, grad_out2, 1,
+                                  (long long)n * voxels, grad_logits, stream);
 }
 
 int mdt_seg_loss_weighted_forward(const float *logits, const long long *strides3, const unsigned char *target, int n, long long voxels, int n_classes,
@@ -513,8 +644,86 @@ int mdt_seg_loss_weighted_backward(const float *logits, const long long *strides
                                    float false_positive_weight, float smooth, const float *class_weights, const double *sums, const float *grad_out2,
                                    float *grad_logits, void *stream) {
     if (!class_weights) return MDT_EINVAL;
+    return mdt::seg_loss_backward(logits, strides3, target, n, voxels, n_classes, false_positive_weight, smooth, class_weights, sums, grad_out2, 1,
+                                  (long long)n * voxels, grad_logits, stream);
+}
+
+int mdt_exchange_fill(void *buf, long long count, int f64, void *stream) {
+    if (count < 0 || (count > 0 && !buf) || ((uintptr_t)buf & (f64 ? 7 : 3))) return MDT_EINVAL;
+    if (count == 0) return MDT_OK;
+    const long long blocks = mdt::ceil_div(count, 256LL);
+    mdt::neg_zero_fill_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, mdt::as_stream(stream)>>>(buf, count, f64);
+    return mdt::launch_status();
+}
+
+size_t mdt_seg_loss_sample_workspace_bytes(int n, long long voxels, int n_classes) {
+    if (n < 1 || voxels < 1 || n_classes < 1 || n_classes > mdt::kMaxCls || (long long)n * mdt::seg_sample_chunks(voxels) >= (1LL << 31)) return 0;
+    return (size_t)n * mdt::seg_sample_chunks(voxels) * (3 * n_classes + 1) * sizeof(double);
+}
+
+}  // extern "C"
+
+namespace mdt {
+
+static int seg_loss_sample_sums(const float *logits, const long long *strides3, const unsigned char *target, int n, long long voxels, int n_classes,
+                                const float *class_weights, double *rows, void *ws, size_t ws_bytes, void *stream) {
+    if (!logits || !strides3 || !target || !rows || !ws || n <= 0 || voxels <= 0) return MDT_EINVAL;
+    if (n_classes < 1 || n_classes > kMaxCls) return MDT_EUNSUPPORTED;
+    const size_t need = mdt_seg_loss_sample_workspace_bytes(n, voxels, n_classes);
+    if (need == 0) return MDT_EINVAL;
+    if (ws_bytes < need) return MDT_EWORKSPACE;
+    SegGeom g{n, n_classes, voxels, strides3[0], strides3[1], strides3[2]};
+    const int chunks = seg_sample_chunks(voxels), nv = 3 * n_classes + 1;
+    cudaStream_t st = as_stream(stream);
+    double *partial = reinterpret_cast<double *>(ws);
+    if (class_weights)
+        seg_sample_partials_kernel<true><<<(unsigned)(n * chunks), 256, 0, st>>>(logits, target, g, chunks, class_weights, partial);
+    else
+        seg_sample_partials_kernel<false><<<(unsigned)(n * chunks), 256, 0, st>>>(logits, target, g, chunks, nullptr, partial);
+    int e = launch_status();
+    if (e) return e;
+    seg_sample_rows_kernel<<<(unsigned)ceil_div<long long>((long long)n * nv * 32, 256), 256, 0, st>>>(partial, n, chunks, nv, rows);
+    return launch_status();
+}
+
+}  // namespace mdt
+
+extern "C" {
+
+int mdt_seg_loss_sample_sums(const float *logits, const long long *strides3, const unsigned char *target, int n, long long voxels, int n_classes,
+                             double *rows, void *ws, size_t ws_bytes, void *stream) {
+    return mdt::seg_loss_sample_sums(logits, strides3, target, n, voxels, n_classes, nullptr, rows, ws, ws_bytes, stream);
+}
+
+int mdt_seg_loss_weighted_sample_sums(const float *logits, const long long *strides3, const unsigned char *target, int n, long long voxels,
+                                      int n_classes, const float *class_weights, double *rows, void *ws, size_t ws_bytes, void *stream) {
+    if (!class_weights) return MDT_EINVAL;
+    return mdt::seg_loss_sample_sums(logits, strides3, target, n, voxels, n_classes, class_weights, rows, ws, ws_bytes, stream);
+}
+
+int mdt_seg_loss_from_sums(const double *rows, int n_total, long long voxels, int n_classes, float false_positive_weight, float smooth,
+                           const float *class_weights, double *sums, float *out2, void *stream) {
+    if (!rows || !sums || !out2 || n_total <= 0 || voxels <= 0) return MDT_EINVAL;
+    if (n_classes < 1 || n_classes > mdt::kMaxCls) return MDT_EUNSUPPORTED;
+    mdt::seg_from_sums_kernel<<<1, 32, 0, mdt::as_stream(stream)>>>(rows, n_total, voxels, n_classes, false_positive_weight, smooth, class_weights, sums,
+                                                                    out2);
+    return mdt::launch_status();
+}
+
+int mdt_seg_loss_backward_global(const float *logits, const long long *strides3, const unsigned char *target, int n, long long voxels, int n_classes,
+                                 float false_positive_weight, float smooth, const double *sums, long long total_voxels, const float *grad_out2,
+                                 int n_ranks, float *grad_logits, void *stream) {
+    return mdt::seg_loss_backward(logits, strides3, target, n, voxels, n_classes, false_positive_weight, smooth, nullptr, sums, grad_out2, n_ranks,
+                                  total_voxels, grad_logits, stream);
+}
+
+int mdt_seg_loss_weighted_backward_global(const float *logits, const long long *strides3, const unsigned char *target, int n, long long voxels,
+                                          int n_classes, float false_positive_weight, float smooth, const float *class_weights, const double *sums,
+                                          long long total_voxels, const float *grad_out2, int n_ranks, float *grad_logits,
+                                          void *stream) {
+    if (!class_weights) return MDT_EINVAL;
     return mdt::seg_loss_backward(logits, strides3, target, n, voxels, n_classes, false_positive_weight, smooth, class_weights, sums, grad_out2,
-                                  grad_logits, stream);
+                                  n_ranks, total_voxels, grad_logits, stream);
 }
 
 size_t mdt_shem_workspace_bytes(int n_anchors, int k_pool) {

@@ -244,6 +244,76 @@ __global__ void __launch_bounds__(256) act_bwd_kernel(const float *__restrict__ 
         dx[i] = dy[i] * act_grad(y[i], act, slope);
 }
 
+// ---------------------------------------------------------------------------------------------------- per-sample sums (batch norm across ranks)
+// The sums of one sample must not depend on which batch it sits in, so the row split of a sample is a function of (s, c) only: up to
+// kSampleChunks blocks per sample (wide enough that a batch of one still fills the SMs), no block below kMinBlockElems elements.
+constexpr long long kSampleChunks = 512;
+
+bool make_sample_geo(int n, long long s, int c, Geo &g) {
+    if (n < 1 || s < 1 || c < 1 || (long long)n * s > (1LL << 40) / c) return false;
+    g.B = n;
+    g.C = c;
+    g.R = s;
+    const long long min_rows = kMinBlockElems / c > 0 ? kMinBlockElems / c : 1;
+    long long chunks = ceil_div(s, min_rows);
+    chunks = chunks < kSampleChunks ? chunks : kSampleChunks;
+    g.rows = ceil_div(s, chunks);
+    g.chunks = (int)ceil_div(s, g.rows);
+    return (long long)g.B * g.chunks < (1LL << 31);
+}
+
+// BwdLoad with per-channel statistics (batch norm) over a per-sample walk, whose group index is (sample, channel)
+struct ChannelBwdLoad {
+    BwdLoad l;
+    int C;
+    __device__ double2 operator()(long long i, int grp) const { return l(i, grp % C); }
+};
+
+// rows [N][C] in sample order -> per-channel statistics over M = N * s rows (the finalisation of stats_finalize_kernel)
+__global__ void stats_from_sums_kernel(const double2 *__restrict__ rows, int N, long long s, int C, float eps, float momentum,
+                                       float *__restrict__ mean, float *__restrict__ rstd, float *__restrict__ running_mean,
+                                       float *__restrict__ running_var, long long *__restrict__ num_batches_tracked) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    double sa = 0.0, sb = 0.0;
+    for (int b = 0; b < N; ++b) {
+        const double2 v = rows[(long long)b * C + c];
+        sa += v.x;
+        sb += v.y;
+    }
+    const double M = (double)N * (double)s, mu = sa / M;
+    double var = sb / M - mu * mu;
+    var = var > 0.0 ? var : 0.0;
+    mean[c] = (float)mu;
+    rstd[c] = (float)(1.0 / sqrt(var + (double)eps));
+    if (running_mean != nullptr) {
+        const double m = momentum;
+        running_mean[c] = (float)((1.0 - m) * running_mean[c] + m * mu);
+        running_var[c] = (float)((1.0 - m) * running_var[c] + m * var * (M / (M - 1.0)));
+    }
+    if (num_batches_tracked != nullptr && c == 0) *num_batches_tracked += 1;
+}
+
+// global rows [N][C] (sum g, sum g xhat) -> totals[c] over all rows in order; dgamma / dbeta over the local rows [first, first + n) in order
+__global__ void bwd_from_sums_kernel(const double2 *__restrict__ rows, int N, int first, int n, int C, double2 *__restrict__ totals,
+                                     float *__restrict__ dgamma, float *__restrict__ dbeta) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    double sg = 0.0, sgx = 0.0;
+    for (int b = 0; b < N; ++b) {
+        sg += rows[(long long)b * C + c].x;
+        sgx += rows[(long long)b * C + c].y;
+    }
+    totals[c] = make_double2(sg, sgx);
+    sg = sgx = 0.0;
+    for (int b = first; b < first + n; ++b) {
+        sg += rows[(long long)b * C + c].x;
+        sgx += rows[(long long)b * C + c].y;
+    }
+    if (dgamma != nullptr) dgamma[c] = (float)sgx;
+    if (dbeta != nullptr) dbeta[c] = (float)sg;
+}
+
 bool aligned4(const void *p) { return ((uintptr_t)p & 3) == 0; }
 bool act_ok(int act, float slope) { return act >= 0 && act <= 2 && slope == slope; }
 int finalize_grid(const Geo &g) { return (int)ceil_div((long long)g.B * g.C * 32, (long long)kThreads); }
@@ -323,6 +393,75 @@ int mdt_norm_backward(const float *dy, const float *y, const float *x, const flo
         }
     }
     const BwdApplyOp op{dy, y, x, mean, rstd, gamma, batch_stats ? gsum : nullptr, dx, dresidual, (float)(1.0 / (double)g.R), slope, act};
+    rows_kernel<<<g.B * g.chunks, kThreads, 0, st>>>(op, g);
+    return launch_status();
+}
+
+size_t mdt_norm_sample_workspace_bytes(int n, long long s, int c) {
+    Geo g;
+    if (!make_sample_geo(n, s, c, g)) return 0;
+    const size_t part = partial_bytes(g), tot = (size_t)c * sizeof(double2);
+    return part > tot ? part : tot;
+}
+
+int mdt_norm_sample_sums(const float *x, int n, long long s, int c, double *sums, void *ws, size_t ws_bytes, void *stream) {
+    Geo g;
+    if (!make_sample_geo(n, s, c, g) || !x || !sums || !ws || !aligned4(x) || ((uintptr_t)sums & 15) || ((uintptr_t)ws & 15)) return MDT_EINVAL;
+    if (ws_bytes < partial_bytes(g)) return MDT_EWORKSPACE;
+    cudaStream_t st = as_stream(stream);
+    double2 *part = reinterpret_cast<double2 *>(ws);
+    partials_kernel<<<g.B * g.chunks, kThreads, 0, st>>>(StatsLoad{x}, g, part);
+    int e = launch_status();
+    if (e) return e;
+    bwd_finalize_kernel<<<finalize_grid(g), kThreads, 0, st>>>(part, g, reinterpret_cast<double2 *>(sums));
+    return launch_status();
+}
+
+int mdt_norm_stats_from_sums(const double *sums, int n_total, long long s, int c, float eps, float momentum, float *mean, float *rstd,
+                             float *running_mean, float *running_var, long long *num_batches_tracked, void *stream) {
+    if (n_total < 1 || s < 1 || c < 1 || !sums || !mean || !rstd || !(eps >= 0.f) || ((uintptr_t)sums & 15)) return MDT_EINVAL;
+    if (!aligned4(mean) || !aligned4(rstd) || (running_mean == nullptr) != (running_var == nullptr)) return MDT_EINVAL;
+    if (running_mean != nullptr && ((long long)n_total * s < 2 || !aligned4(running_mean) || !aligned4(running_var) || !(momentum >= 0.f && momentum <= 1.f)))
+        return MDT_EINVAL;
+    if (num_batches_tracked != nullptr && ((uintptr_t)num_batches_tracked & 7)) return MDT_EINVAL;
+    stats_from_sums_kernel<<<ceil_div(c, 256), 256, 0, as_stream(stream)>>>(reinterpret_cast<const double2 *>(sums), n_total, s, c, eps, momentum, mean,
+                                                                            rstd, running_mean, running_var, num_batches_tracked);
+    return launch_status();
+}
+
+int mdt_norm_backward_sample_sums(const float *dy, const float *y, const float *x, const float *mean, const float *rstd, int n, long long s, int c,
+                                  int act, float slope, double *sums, void *ws, size_t ws_bytes, void *stream) {
+    Geo g;
+    if (!make_sample_geo(n, s, c, g) || !dy || !x || !mean || !rstd || !sums || !ws || !act_ok(act, slope) || (act != 0 && !y)) return MDT_EINVAL;
+    if (!aligned4(dy) || !aligned4(y) || !aligned4(x) || !aligned4(mean) || !aligned4(rstd) || ((uintptr_t)sums & 15) || ((uintptr_t)ws & 15))
+        return MDT_EINVAL;
+    if (ws_bytes < partial_bytes(g)) return MDT_EWORKSPACE;
+    cudaStream_t st = as_stream(stream);
+    double2 *part = reinterpret_cast<double2 *>(ws);
+    partials_kernel<<<g.B * g.chunks, kThreads, 0, st>>>(ChannelBwdLoad{BwdLoad{dy, y, x, mean, rstd, act, slope}, c}, g, part);
+    int e = launch_status();
+    if (e) return e;
+    bwd_finalize_kernel<<<finalize_grid(g), kThreads, 0, st>>>(part, g, reinterpret_cast<double2 *>(sums));
+    return launch_status();
+}
+
+int mdt_norm_backward_from_sums(const float *dy, const float *y, const float *x, const float *mean, const float *rstd, const float *gamma,
+                                const double *global_sums, int n_total, int local_first_row, int n, long long s, int c, int act, float slope, float *dx,
+                                float *dgamma, float *dbeta, float *dresidual, void *ws, size_t ws_bytes, void *stream) {
+    Geo g;
+    if (!make_geo(n, s, c, 0, g) || !dy || !x || !mean || !rstd || !global_sums || !dx || !ws || !act_ok(act, slope) || (act != 0 && !y)) return MDT_EINVAL;
+    if (n_total < n || local_first_row < 0 || local_first_row > n_total - n) return MDT_EINVAL;
+    if (!aligned4(dy) || !aligned4(y) || !aligned4(x) || !aligned4(mean) || !aligned4(rstd) || !aligned4(gamma) || !aligned4(dx) || !aligned4(dgamma) ||
+        !aligned4(dbeta) || !aligned4(dresidual) || ((uintptr_t)global_sums & 15) || ((uintptr_t)ws & 15))
+        return MDT_EINVAL;
+    if (ws_bytes < (size_t)c * sizeof(double2)) return MDT_EWORKSPACE;
+    cudaStream_t st = as_stream(stream);
+    double2 *totals = reinterpret_cast<double2 *>(ws);
+    bwd_from_sums_kernel<<<ceil_div(c, 256), 256, 0, st>>>(reinterpret_cast<const double2 *>(global_sums), n_total, local_first_row, n, c, totals, dgamma,
+                                                           dbeta);
+    int e = launch_status();
+    if (e) return e;
+    const BwdApplyOp op{dy, y, x, mean, rstd, gamma, totals, dx, dresidual, (float)(1.0 / ((double)n_total * (double)s)), slope, act};
     rows_kernel<<<g.B * g.chunks, kThreads, 0, st>>>(op, g);
     return launch_status();
 }

@@ -72,7 +72,7 @@ class net(Detector):
         w = None
         if 'wce' in cf.seg_loss_mode:
             w = torch.tensor(cf.wce_weights, dtype=torch.float32).to(seg_logits.device, non_blocking=True)
-        dice, ce = native_ops.seg_loss(seg_logits, seg_u8, false_positive_weight=float(cf.fp_dice_weight), class_weights=w)
+        dice, ce = native_ops.seg_loss(seg_logits, seg_u8, false_positive_weight=float(cf.fp_dice_weight), class_weights=w, group=self.seg_loss_group())
         return 1 - dice, ce
 
     def train_forward(self, batch, **kwargs):

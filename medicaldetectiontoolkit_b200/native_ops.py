@@ -9,6 +9,7 @@ import ctypes
 import torch
 
 from . import _lib as L
+from . import parallel as P
 
 
 def nms_sorted(dets_sorted, thresh, dim):
@@ -273,6 +274,26 @@ def _seg_layout(logits):
     return st[0], st[1], sv
 
 
+def _seg_loss_args(logits, target, class_weights):
+    """-> (logits with a collapsible layout, its (batch, class, voxel) strides, n, classes, voxels) after the checks both seg-loss paths share"""
+    lay = _seg_layout(logits)
+    if lay is None:
+        logits = logits.contiguous()
+        lay = _seg_layout(logits)
+    n, c = logits.shape[0], logits.shape[1]
+    vox = 1
+    for s in logits.shape[2:]:
+        vox *= s
+    if target.dtype != torch.uint8 or target.numel() != n * vox or not target.is_contiguous():
+        raise L.MdtError("seg_loss: target must be a contiguous uint8 label map with one entry per voxel")
+    if class_weights is not None:
+        if class_weights.dtype != torch.float32 or class_weights.numel() != c or not class_weights.is_contiguous():
+            raise L.MdtError("seg_loss: class_weights must be a contiguous float32 tensor with one weight per class")
+        if class_weights.device != logits.device:
+            raise L.MdtError("seg_loss: class_weights must be on the logits' device (%s), got %s" % (logits.device, class_weights.device))
+    return logits, lay, n, c, vox
+
+
 class _SegLoss(torch.autograd.Function):
     """(dice score over the batch pseudo-volume, mean voxel cross-entropy) of seg logits vs a uint8 label map, csrc/loss_ops.cu — replaces
     softmax + one-hot + batch_dice + cross_entropy (retina_unet.py:395,446-448; model_utils.py:785-799,833-858) by one pass each way"""
@@ -281,16 +302,7 @@ class _SegLoss(torch.autograd.Function):
     def forward(ctx, logits, target, fpw, smooth, class_weights):
         L.require_cuda(logits, target, class_weights)
         lib = L.load()
-        lay = _seg_layout(logits)
-        if lay is None:
-            logits = logits.contiguous()
-            lay = _seg_layout(logits)
-        n, c = logits.shape[0], logits.shape[1]
-        vox = 1
-        for s in logits.shape[2:]:
-            vox *= s
-        if target.dtype != torch.uint8 or target.numel() != n * vox or not target.is_contiguous():
-            raise L.MdtError("seg_loss: target must be a contiguous uint8 label map with one entry per voxel")
+        logits, lay, n, c, vox = _seg_loss_args(logits, target, class_weights)
         dev = logits.device
         sums = torch.empty(3 * c + 1, dtype=torch.float64, device=dev)
         out = torch.empty(2, dtype=torch.float32, device=dev)
@@ -304,10 +316,6 @@ class _SegLoss(torch.autograd.Function):
                 L.check(lib.mdt_seg_loss_forward(L.ptr(logits), strides, L.ptr(target), n, vox, c, float(fpw), float(smooth), L.ptr(sums), L.ptr(out),
                                                  L.ptr(ws), ws_bytes, L.stream_ptr()))
             else:
-                if class_weights.dtype != torch.float32 or class_weights.numel() != c or not class_weights.is_contiguous():
-                    raise L.MdtError("seg_loss: class_weights must be a contiguous float32 tensor with one weight per class")
-                if class_weights.device != dev:
-                    raise L.MdtError("seg_loss: class_weights must be on the logits' device (%s), got %s" % (dev, class_weights.device))
                 L.check(lib.mdt_seg_loss_weighted_forward(L.ptr(logits), strides, L.ptr(target), n, vox, c, float(fpw), float(smooth), L.ptr(class_weights),
                                                           L.ptr(sums), L.ptr(out), L.ptr(ws), ws_bytes, L.stream_ptr()))
         ctx.save_for_backward(logits, target, sums, class_weights)
@@ -332,11 +340,69 @@ class _SegLoss(torch.autograd.Function):
         return grad, None, None, None, None
 
 
-def seg_loss(seg_logits, seg_labels_u8, false_positive_weight=1.0, smooth=1e-6, class_weights=None):
+class _SyncSegLoss(torch.autograd.Function):
+    """_SegLoss over the batch of all ranks of `group` (the same n on every rank): per-sample sums -> one exchange -> dice and CE of the whole
+    batch on every rank.  Each rank's loss holds the global term once, so the backward sums the incoming gradients over the ranks (the SyncBN
+    rule, done by gathering every rank's incoming pair and adding the pairs in rank order in the kernel): after FlatGradAllReduce averages the
+    parameter gradients, they are the one-GPU gradients of that term."""
+
+    @staticmethod
+    def forward(ctx, logits, target, fpw, smooth, class_weights, group):
+        L.require_cuda(logits, target, class_weights)
+        lib = L.load()
+        logits, lay, n, c, vox = _seg_loss_args(logits, target, class_weights)
+        dev = logits.device
+        ws_bytes = lib.mdt_seg_loss_sample_workspace_bytes(n, vox, c)
+        if ws_bytes == 0:
+            raise L.MdtError("seg_loss: at most 8 classes")
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        sums = torch.empty(3 * c + 1, dtype=torch.float64, device=dev)
+        out = torch.empty(2, dtype=torch.float32, device=dev)
+        strides = L.i64arr(lay)
+        with torch.cuda.device(dev):
+            buf, slot = P.row_slots(n, 3 * c + 1, dev, group)
+            if class_weights is None:
+                L.check(lib.mdt_seg_loss_sample_sums(L.ptr(logits), strides, L.ptr(target), n, vox, c, L.ptr(slot), L.ptr(ws), ws_bytes, L.stream_ptr()))
+            else:
+                L.check(lib.mdt_seg_loss_weighted_sample_sums(L.ptr(logits), strides, L.ptr(target), n, vox, c, L.ptr(class_weights), L.ptr(slot),
+                                                              L.ptr(ws), ws_bytes, L.stream_ptr()))
+            rows = P.all_reduce_rows(buf, group)
+            L.check(lib.mdt_seg_loss_from_sums(L.ptr(rows), rows.shape[0], vox, c, float(fpw), float(smooth), L.ptr(class_weights), L.ptr(sums),
+                                               L.ptr(out), L.stream_ptr()))
+        ctx.save_for_backward(logits, target, sums, class_weights)
+        ctx.meta = (lay, n, vox, c, float(fpw), float(smooth), rows.shape[0] * vox, group)
+        return out[0], out[1]
+
+    @staticmethod
+    def backward(ctx, g_dice, g_ce):
+        lib = L.load()
+        logits, target, sums, class_weights = ctx.saved_tensors
+        lay, n, vox, c, fpw, smooth, total, group = ctx.meta
+        zero = logits.new_zeros(())                      # an output that did not enter the loss arrives as None
+        grad = torch.empty_strided(logits.shape, logits.stride(), dtype=torch.float32, device=logits.device)
+        with torch.cuda.device(logits.device):
+            # every rank's {dL/d dice, dL/d ce} in rank order: the kernel adds them in fp64 in that order
+            buf, slot = P.row_slots(1, 2, logits.device, group, dtype=torch.float32)
+            torch.stack([(g if g is not None else zero).reshape(()) for g in (g_dice, g_ce)], out=slot[0])
+            gout = P.all_reduce_rows(buf, group)
+            if class_weights is None:
+                L.check(lib.mdt_seg_loss_backward_global(L.ptr(logits), L.i64arr(lay), L.ptr(target), n, vox, c, fpw, smooth, L.ptr(sums), total,
+                                                         L.ptr(gout), gout.shape[0], L.ptr(grad), L.stream_ptr()))
+            else:
+                L.check(lib.mdt_seg_loss_weighted_backward_global(L.ptr(logits), L.i64arr(lay), L.ptr(target), n, vox, c, fpw, smooth, L.ptr(class_weights),
+                                                                  L.ptr(sums), total, L.ptr(gout), gout.shape[0], L.ptr(grad), L.stream_ptr()))
+        return grad, None, None, None, None, None
+
+
+def seg_loss(seg_logits, seg_labels_u8, false_positive_weight=1.0, smooth=1e-6, class_weights=None, group=None):
     """-> (batch_dice(softmax(seg_logits), one_hot(labels)), cross_entropy(seg_logits, labels)), both differentiable 0-d tensors.
-    class_weights: optional per-class weights of the cross-entropy on the logits' device (F.cross_entropy(weight=)); the dice term is unchanged"""
+    class_weights: optional per-class weights of the cross-entropy on the logits' device (F.cross_entropy(weight=)); the dice term is unchanged.
+    group: a process group whose ranks hold the rest of the batch (the same batch size on every rank): dice and CE are then those of the whole
+    batch, in rank order, on every rank, and every rank must run this loss's backward"""
     if seg_logits.dtype != torch.float32:
         raise L.MdtError("seg_loss: logits must be float32")
+    if group is not None:
+        return _SyncSegLoss.apply(seg_logits, seg_labels_u8, false_positive_weight, smooth, class_weights, group)
     return _SegLoss.apply(seg_logits, seg_labels_u8, false_positive_weight, smooth, class_weights)
 
 

@@ -5,12 +5,16 @@ The modules subclass torch's, so parameters, buffers (`weight`, `bias`, `running
 load_state_dict, train() / eval() and isinstance checks are exactly the reference's.  Only `forward` differs: one statistics pass and one
 apply pass that also runs the following activation (and, inside a ResBlock, the residual add), all on channels-last maps.  Options the conv
 factory never builds raise instead of running on a torch kernel; there is no CPU fallback.
+
+A batch norm with `process_group` set (parallel.sync_batch_statistics) takes its training-mode statistics over the batch of all the group's
+ranks: per-sample fp64 sums, one exchange of those rows, and the statistics added up in rank order (the same bits at any world size).
 """
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _lib as L
+from . import parallel as P
 from .conv import _workspace
 
 ACTS = {None: 0, 'relu': 1, 'leaky_relu': 2}
@@ -71,6 +75,59 @@ class _NormActFn(torch.autograd.Function):
                                           LEAKY_SLOPE, int(batch_stats), L.ptr(dx), L.ptr(dw), L.ptr(db), L.ptr(dres), L.ptr(ws), ws.numel(),
                                           L.stream_ptr()))
         return dx, dw, db, dres, None, None, None, None, None, None, None, None
+
+
+class _SyncBatchNormActFn(torch.autograd.Function):
+    """_NormActFn for batch norm in training mode with the batch split across the ranks of `group`: per-sample sums -> one exchange ->
+    statistics of the whole batch, and the same for the backward.  Every rank must pass the same n."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, residual, running_mean, running_var, num_batches_tracked, momentum, eps, act, group):
+        lib = L.load()
+        L.require_cuda(x, weight, bias, residual, running_mean, running_var)
+        x, fmt = _cl(x)
+        if residual is not None:
+            residual = residual.contiguous(memory_format=fmt)
+        n, c = x.shape[0], x.shape[1]
+        s = x[0, 0].numel()
+        mean = torch.empty(c, dtype=torch.float32, device=x.device)
+        rstd = torch.empty_like(mean)
+        y = torch.empty_like(x, memory_format=fmt)
+        with torch.cuda.device(x.device):
+            ws = _workspace(lib.mdt_norm_sample_workspace_bytes(n, s, c), x.device)
+            buf, slot = P.row_slots(n, 2 * c, x.device, group)
+            L.check(lib.mdt_norm_sample_sums(L.ptr(x), n, s, c, L.ptr(slot), L.ptr(ws), ws.numel(), L.stream_ptr()))
+            rows = P.all_reduce_rows(buf, group)
+            L.check(lib.mdt_norm_stats_from_sums(L.ptr(rows), rows.shape[0], s, c, eps, momentum, L.ptr(mean), L.ptr(rstd), L.ptr(running_mean),
+                                                 L.ptr(running_var), L.ptr(num_batches_tracked), L.stream_ptr()))
+            L.check(lib.mdt_norm_apply(L.ptr(x), L.ptr(mean), L.ptr(rstd), L.ptr(weight), L.ptr(bias), L.ptr(residual), n, s, c, 0, ACTS[act],
+                                       LEAKY_SLOPE, L.ptr(y), L.stream_ptr()))
+        ctx.save_for_backward(x, y if act is not None else None, mean, rstd, weight)
+        ctx.cfg = (fmt, act, bias is not None, residual is not None, group)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        lib = L.load()
+        x, y, mean, rstd, weight = ctx.saved_tensors
+        fmt, act, has_bias, has_res, group = ctx.cfg
+        dy = dy.contiguous(memory_format=fmt)
+        n, c = x.shape[0], x.shape[1]
+        s = x[0, 0].numel()
+        dx = torch.empty_like(x, memory_format=fmt)
+        dw = torch.empty(c, dtype=torch.float32, device=x.device) if weight is not None and ctx.needs_input_grad[1] else None
+        db = torch.empty(c, dtype=torch.float32, device=x.device) if has_bias and ctx.needs_input_grad[2] else None
+        dres = torch.empty_like(x, memory_format=fmt) if has_res and ctx.needs_input_grad[3] else None
+        with torch.cuda.device(x.device):
+            ws = _workspace(lib.mdt_norm_sample_workspace_bytes(n, s, c), x.device)
+            buf, slot = P.row_slots(n, 2 * c, x.device, group)
+            L.check(lib.mdt_norm_backward_sample_sums(L.ptr(dy), L.ptr(y), L.ptr(x), L.ptr(mean), L.ptr(rstd), n, s, c, ACTS[act], LEAKY_SLOPE,
+                                                      L.ptr(slot), L.ptr(ws), ws.numel(), L.stream_ptr()))
+            rows = P.all_reduce_rows(buf, group)
+            L.check(lib.mdt_norm_backward_from_sums(L.ptr(dy), L.ptr(y), L.ptr(x), L.ptr(mean), L.ptr(rstd), L.ptr(weight), L.ptr(rows), rows.shape[0],
+                                                    P.dist.get_rank(group) * n, n, s, c, ACTS[act], LEAKY_SLOPE, L.ptr(dx), L.ptr(dw), L.ptr(db),
+                                                    L.ptr(dres), L.ptr(ws), ws.numel(), L.stream_ptr()))
+        return dx, dw, db, dres, None, None, None, None, None, None, None
 
 
 class _ActFn(torch.autograd.Function):
@@ -143,6 +200,9 @@ class _NativeNorm:
             F._verify_spatial_size(input.size())
             return _NormActFn.apply(input, None, None, residual, None, None, None, True, True, self.momentum, self.eps, act)
         batch_stats = self.training
+        if batch_stats and self.process_group is not None:
+            return _SyncBatchNormActFn.apply(input, self.weight, self.bias, residual, self.running_mean, self.running_var, self.num_batches_tracked,
+                                             self.momentum, self.eps, act, self.process_group)
         if batch_stats:
             F._verify_batch_size(input.size())
         return _NormActFn.apply(input, self.weight, self.bias, residual, self.running_mean, self.running_var,
@@ -177,6 +237,9 @@ class InstanceNorm2d(_NativeInstanceNorm, nn.InstanceNorm2d):
 
 
 class _NativeBatchNorm(_NativeNorm):
+    # set by parallel.sync_batch_statistics: in training mode the statistics are then those of the whole batch across the group's ranks
+    process_group = None
+
     def _init_check(self, affine, track_running_stats, momentum, dtype):
         if not (affine and track_running_stats):
             raise ValueError("%s: affine=False / track_running_stats=False are not supported by the native kernels (the conv factory builds "

@@ -306,7 +306,7 @@ class net(Detector):
         batch_class_loss, batch_bbox_loss, monitor = anchor_losses(matched, class_logits, pred_deltas, cf, compute_class_loss, compute_bbox_loss)
         loss = batch_class_loss + batch_bbox_loss
         if self.has_seg_head:
-            seg_dice, seg_ce = seg_loss_terms(seg_logits, seg, cf)
+            seg_dice, seg_ce = seg_loss_terms(seg_logits, seg, cf, group=self.seg_loss_group())
             loss = loss + (seg_dice + seg_ce) / 2
 
         detections = self._detect(class_logits, pred_deltas)

@@ -100,7 +100,7 @@ class net(Detector):
                                                                compute_rpn_bbox_loss)
         mrcnn_class_loss = compute_mrcnn_class_loss(t_cls, logits)
         mrcnn_bbox_loss = compute_mrcnn_bbox_loss(t_deltas, pred_deltas, t_cls)
-        seg_dice, seg_ce = seg_loss_terms(seg_logits, seg, cf)
+        seg_dice, seg_ce = seg_loss_terms(seg_logits, seg, cf, group=self.seg_loss_group())
         loss = rpn_class_loss + rpn_bbox_loss + mrcnn_class_loss + mrcnn_bbox_loss + (seg_dice + seg_ce) / 2
         detections = self._detect(refine_args)
 
