@@ -67,7 +67,9 @@ int mdt_crop_and_resize_3d_forward(const float *image, const int64_t *img_stride
                                    int batch, int image_height, int image_width, int image_zdepth, int crop_height, int crop_width,
                                    int crop_zdepth, int depth, float extrapolation_value, float *crops, const int64_t *crop_strides_host,
                                    void *stream);
-/* grads_image must be zero-filled by the caller OR pass zero_init=1 to have the library memset it (contiguous-in-memory extent given by image_numel) */
+/* backward: a gather in a fixed order (csrc/roi_align.cu), so two calls with the same arguments give the same bits.  Every logical element of
+ * grads_image is written once: zero_init=1 gives the sum of the RoI terms, zero_init=0 adds them to the element's prior content; elements between
+ * strided rows are not touched.  image_numel (> 0 with zero_init=1) is the caller's extent of grads_image, as before. */
 int mdt_crop_and_resize_3d_backward(const float *grads, const int64_t *grad_strides_host, const float *boxes, const int *box_ind, int num_boxes,
                                     int batch, int image_height, int image_width, int image_zdepth, int crop_height, int crop_width,
                                     int crop_zdepth, int depth, float *grads_image, const int64_t *img_strides_host, int zero_init,
@@ -84,7 +86,8 @@ int mdt_crop_and_resize_2d_backward(const float *grads, const int64_t *grad_stri
  * round(4 + log2(sqrt(h*w))) rule is evaluated by the caller); every crop row is written exactly once, bad box_ind rows are zeros.
  * images / grad_images: HOST arrays of nlevels device pointers (channels-last maps, C % 4 == 0); image_strides: nlevels x 5 int64 element strides
  * (b, c, y, x, z); image_dims: nlevels x 3 (H, W, Z).  Returns MDT_EUNSUPPORTED for layouts outside the vector kernel (caller then loops over
- * levels with mdt_crop_and_resize_*).  dim = 2 or 3 (2: crop_zdepth and the Z entries are ignored). */
+ * levels with mdt_crop_and_resize_*).  dim = 2 or 3 (2: crop_zdepth and the Z entries are ignored).  The backward is the single-map entry
+ * point's gather, each level's map receiving its own RoIs (image_numel: nlevels extents, > 0 with zero_init=1). */
 int mdt_pyramid_roi_align_forward(int dim, const float *const *images, const int64_t *image_strides, const int *image_dims, int nlevels, const float *boxes,
                                   const int *box_ind, const int *roi_level, int num_boxes, int batch, int crop_height, int crop_width, int crop_zdepth,
                                   int depth, float *crops, const int64_t *crop_strides, void *stream);

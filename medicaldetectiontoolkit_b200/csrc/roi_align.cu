@@ -3,14 +3,17 @@
 // Reference semantics followed (paths relative to the reference root):
 //   sampling coordinates  cuda_functions/roi_align_3D/roi_align/src/cuda/crop_and_resize_kernel.cu:52-106 ("fixed" half-bin-centred, clamped to the map)
 //   neighbours / lerp     :110-147   forward interpolation order (x, then y, then z)
-//   backward weights      :256-301   8 (2D: 4) scatter-adds into a zero-initialised image gradient
+//   backward weights      :256-301   8 (2D: 4) weighted terms per bin (the reference scatters them with atomics; here each image-gradient
+//                                    element gathers its terms in a fixed order, see roi_bwd_gather)
 //   bad box_ind           :43-47 + crop_and_resize_gpu.c:27: that crop is all zeros
 //   2D twin               cuda_functions/roi_align_2D/roi_align/src/cuda/crop_and_resize_kernel.cu:10-194
 //
 // Design: the reference runs one thread per output scalar over an NCDHW map, so the 8 gathers of a warp hit 8x32 different
-// sectors. Here the fast path works on channels-last maps (the layout the tensor-core conv kernels produce): one thread owns one bin x 4
-// channels, so every corner read / gradient scatter of a warp is a run of consecutive 16-byte vectors (fully coalesced 128-bit
-// ld.global.nc / red.global.add.v4.f32). A stride-generic scalar kernel keeps the reference's NCDHW contract working with no copy.
+// sectors. Here the fast forward path works on channels-last maps (the layout the tensor-core conv kernels produce): one thread owns one
+// bin x 4 channels, so every corner read of a warp is a run of consecutive 16-byte vectors (fully coalesced 128-bit ld.global.nc). A
+// stride-generic scalar kernel keeps the reference's NCDHW contract working with no copy.
+#include <algorithm>
+
 #include "mdt_common.cuh"
 
 namespace mdt {
@@ -87,39 +90,6 @@ __global__ void __launch_bounds__(256) roi_fwd_scalar(RoiGeom g, const float *__
     }
 }
 
-template <int DIM, typename IdxT>
-__global__ void __launch_bounds__(256) roi_bwd_scalar(RoiGeom g, const float *__restrict__ grads, const float *__restrict__ boxes,
-                                                     const int *__restrict__ box_ind, float *__restrict__ gimg, int c_fastest, long long total) {
-    for (IdxT t = blockIdx.x * (IdxT)blockDim.x + threadIdx.x; t < (IdxT)total; t += (IdxT)gridDim.x * blockDim.x) {
-        IdxT r = t;
-        int c, z, x, y;
-        if (c_fastest) { c = r % g.C; r /= g.C; z = r % g.cz; r /= g.cz; x = r % g.cw; r /= g.cw; y = r % g.ch; r /= g.ch; }
-        else           { z = r % g.cz; r /= g.cz; x = r % g.cw; r /= g.cw; y = r % g.ch; r /= g.ch; c = r % g.C; r /= g.C; }
-        const int n = (int)r;
-        Tap ty, tx, tz; int b;
-        if (!bin_taps<DIM>(g, boxes, box_ind, n, y, x, z, ty, tx, tz, b)) continue;
-        const float gv = grads[n * g.os[0] + c * g.os[1] + y * g.os[2] + x * g.os[3] + z * g.os[4]];
-        float *p = gimg + b * g.is[0] + c * g.is[1];
-#pragma unroll
-        for (int kz = 0; kz < (DIM == 3 ? 2 : 1); ++kz) {
-            const float wz = (DIM == 3) ? (kz ? tz.lerp : 1 - tz.lerp) : 1.f;
-            const int64_t oz = (DIM == 3) ? (kz ? tz.hi : tz.lo) * g.is[4] : 0;
-#pragma unroll
-            for (int ky = 0; ky < 2; ++ky) {
-                const float wy = ky ? ty.lerp : 1 - ty.lerp;
-                const int64_t oy = (ky ? ty.hi : ty.lo) * g.is[2];
-#pragma unroll
-                for (int kx = 0; kx < 2; ++kx) {
-                    const float wx = kx ? tx.lerp : 1 - tx.lerp;
-                    // weight product order of the reference: x * z * y * grad
-                    const float w = (DIM == 3) ? wx * wz * wy * gv : wx * wy * gv;
-                    if (w != 0.f) atomicAdd(p + oy + (kx ? tx.hi : tx.lo) * g.is[3] + oz, w);
-                }
-            }
-        }
-    }
-}
-
 // ---------------------------------------------------------------- channels-last float4 kernels ----------------------------------------------------------------
 // requires is[1] == 1, os[1] == 1, C % 4 == 0, all other strides % 4 == 0 and 16-byte aligned bases.
 template <int DIM, typename IdxT>
@@ -158,42 +128,6 @@ __global__ void __launch_bounds__(256) roi_fwd_cl4(RoiGeom g, const float *__res
     }
 }
 
-template <int DIM, typename IdxT>
-__global__ void __launch_bounds__(256) roi_bwd_cl4(RoiGeom g, const float *__restrict__ grads, const float *__restrict__ boxes,
-                                                  const int *__restrict__ box_ind, float *__restrict__ gimg, long long total) {
-    const int C4 = g.C >> 2;
-    for (IdxT t = blockIdx.x * (IdxT)blockDim.x + threadIdx.x; t < (IdxT)total; t += (IdxT)gridDim.x * blockDim.x) {
-        IdxT r = t;
-        const int c4 = r % C4; r /= C4;
-        const int z = r % g.cz; r /= g.cz;
-        const int x = r % g.cw; r /= g.cw;
-        const int y = r % g.ch; r /= g.ch;
-        const int n = (int)r;
-        Tap ty, tx, tz; int b;
-        if (!bin_taps<DIM>(g, boxes, box_ind, n, y, x, z, ty, tx, tz, b)) continue;
-        const float4 gv = __ldg(reinterpret_cast<const float4 *>(grads + n * g.os[0] + y * g.os[2] + x * g.os[3] + z * g.os[4]) + c4);
-        float *p = gimg + b * g.is[0] + 4 * c4;
-#pragma unroll
-        for (int kz = 0; kz < (DIM == 3 ? 2 : 1); ++kz) {
-            const float wz = (DIM == 3) ? (kz ? tz.lerp : 1 - tz.lerp) : 1.f;
-            const int64_t oz = (DIM == 3) ? (kz ? tz.hi : tz.lo) * g.is[4] : 0;
-#pragma unroll
-            for (int ky = 0; ky < 2; ++ky) {
-                const float wy = ky ? ty.lerp : 1 - ty.lerp;
-                const int64_t oy = (ky ? ty.hi : ty.lo) * g.is[2];
-#pragma unroll
-                for (int kx = 0; kx < 2; ++kx) {
-                    const float wx = kx ? tx.lerp : 1 - tx.lerp;
-                    const float w = (DIM == 3) ? wx * wz * wy : wx * wy;
-                    if (w != 0.f)  // one 128-bit reduction (RED.E.ADD.F32x4) instead of four scalar atomics
-                        atomicAdd(reinterpret_cast<float4 *>(p + oy + (kx ? tx.hi : tx.lo) * g.is[3] + oz),
-                                  make_float4(w * gv.x, w * gv.y, w * gv.z, w * gv.w));
-                }
-            }
-        }
-    }
-}
-
 // ---------------------------------------------------------------- channels-last, one RoI (slice) per CTA ----------------------------------------------------------------
 // ncu of roi_fwd_cl4 (P2, 7x7x3, 1024 RoIs): 390 instructions per thread, issue slots 54 % busy, DRAM 10 %: every one of the C/4
 // threads of a bin repeats the index decomposition (five integer divisions), three sampling coordinates (a float division each) and
@@ -202,7 +136,7 @@ __global__ void __launch_bounds__(256) roi_bwd_cl4(RoiGeom g, const float *__res
 // 3 per bin.  A CTA therefore owns one RoI (or a slice of its bins when the crop is large): ch+cw+cz threads compute one tap each
 // (neighbour offsets + lerp weight; box and box_ind loads are independent of each other), one pass fills a per-bin table (packed tap
 // indices + output offset), and then all 256 threads stream (bin, 4-channel) items: table lookups, eight 128-bit gathers, lerp, one
-// 128-bit store - no divisions and no barrier in the loop.  Expressions are those of roi_fwd_cl4 / roi_bwd_cl4: bit-identical results.
+// 128-bit store - no divisions and no barrier in the loop.  Expressions are those of roi_fwd_cl4: bit-identical results.
 constexpr int kRoiThreads = 256;
 constexpr int kMaxCropDim = 64;       // per axis, for the shared-memory tap tables
 constexpr int kMaxBinsPerCta = 1024;  // bins per CTA slice (12 KB of tables)
@@ -214,7 +148,7 @@ struct RoiTables {
     int yxz[kMaxBinsPerCta];                      // y | x << 8 | z << 16
 };
 
-template <int DIM, bool BWD>
+template <int DIM>
 __device__ __forceinline__ void roi_cl4_per_roi_body(const RoiGeom &g, const float *__restrict__ src, const float *__restrict__ boxes,
                                                      const int *__restrict__ box_ind, float *__restrict__ dst, int bins_per_slice, RoiTables &s) {
     const int n = blockIdx.x, tid = threadIdx.x;
@@ -245,87 +179,64 @@ __device__ __forceinline__ void roi_cl4_per_roi_body(const RoiGeom &g, const flo
     const int items = nbins * C4;
     int bl = tid / C4, c4 = tid - bl * C4;                        // item -> (bin, channel group), advanced without divisions
     const int dq = kRoiThreads / C4, dr = kRoiThreads - dq * C4;
-    const float *img = BWD ? nullptr : src + (valid ? b_in : 0) * g.is[0];
-    float *gim = BWD ? dst + (valid ? b_in : 0) * g.is[0] : nullptr;
+    const float *img = src + (valid ? b_in : 0) * g.is[0];
     for (int item = tid; item < items; item += kRoiThreads) {
         const long long out_off = s.out[bl];
         if (!valid) {
-            if (!BWD) *(reinterpret_cast<float4 *>(dst + out_off) + c4) = make_float4(0.f, 0.f, 0.f, 0.f);
+            *(reinterpret_cast<float4 *>(dst + out_off) + c4) = make_float4(0.f, 0.f, 0.f, 0.f);
         } else {
             const int pk = s.yxz[bl];
             const int y = pk & 255, x = (pk >> 8) & 255, z = pk >> 16;
             const int ylo = s.lo[0][y], yhi = s.hi[0][y], xlo = s.lo[1][x], xhi = s.hi[1][x];
             const float ly = s.lerp[0][y], lx = s.lerp[1][x], lz = (DIM == 3) ? s.lerp[2][z] : 0.f;
-            if (!BWD) {
-                const float *p = img + 4 * c4;
-                float4 v[2];
+            const float *p = img + 4 * c4;
+            float4 v[2];
 #pragma unroll
-                for (int kz = 0; kz < (DIM == 3 ? 2 : 1); ++kz) {
-                    const int oz = (DIM == 3) ? (kz ? s.hi[2][z] : s.lo[2][z]) : 0;
-                    const float4 tl = __ldg(reinterpret_cast<const float4 *>(p + ylo + xlo + oz));
-                    const float4 tr = __ldg(reinterpret_cast<const float4 *>(p + ylo + xhi + oz));
-                    const float4 bl_ = __ldg(reinterpret_cast<const float4 *>(p + yhi + xlo + oz));
-                    const float4 br = __ldg(reinterpret_cast<const float4 *>(p + yhi + xhi + oz));
+            for (int kz = 0; kz < (DIM == 3 ? 2 : 1); ++kz) {
+                const int oz = (DIM == 3) ? (kz ? s.hi[2][z] : s.lo[2][z]) : 0;
+                const float4 tl = __ldg(reinterpret_cast<const float4 *>(p + ylo + xlo + oz));
+                const float4 tr = __ldg(reinterpret_cast<const float4 *>(p + ylo + xhi + oz));
+                const float4 bl_ = __ldg(reinterpret_cast<const float4 *>(p + yhi + xlo + oz));
+                const float4 br = __ldg(reinterpret_cast<const float4 *>(p + yhi + xhi + oz));
 #define MDT_LERP2(f) { const float top = tl.f + (tr.f - tl.f) * lx, bot = bl_.f + (br.f - bl_.f) * lx; v[kz].f = top + (bot - top) * ly; }
-                    MDT_LERP2(x) MDT_LERP2(y) MDT_LERP2(z) MDT_LERP2(w)
+                MDT_LERP2(x) MDT_LERP2(y) MDT_LERP2(z) MDT_LERP2(w)
 #undef MDT_LERP2
-                }
-                float4 o = v[0];
-                if (DIM == 3) {
-                    o.x = v[0].x + (v[1].x - v[0].x) * lz; o.y = v[0].y + (v[1].y - v[0].y) * lz;
-                    o.z = v[0].z + (v[1].z - v[0].z) * lz; o.w = v[0].w + (v[1].w - v[0].w) * lz;
-                }
-                *(reinterpret_cast<float4 *>(dst + out_off) + c4) = o;
-            } else {
-                const float4 gv = __ldg(reinterpret_cast<const float4 *>(src + out_off) + c4);
-                float *p = gim + 4 * c4;
-#pragma unroll
-                for (int kz = 0; kz < (DIM == 3 ? 2 : 1); ++kz) {
-                    const float wz = (DIM == 3) ? (kz ? lz : 1 - lz) : 1.f;
-                    const int oz = (DIM == 3) ? (kz ? s.hi[2][z] : s.lo[2][z]) : 0;
-#pragma unroll
-                    for (int ky = 0; ky < 2; ++ky) {
-                        const float wy = ky ? ly : 1 - ly;
-                        const int oy = ky ? yhi : ylo;
-#pragma unroll
-                        for (int kx = 0; kx < 2; ++kx) {
-                            const float wx = kx ? lx : 1 - lx;
-                            const float w = (DIM == 3) ? wx * wz * wy : wx * wy;
-                            if (w != 0.f)  // one 128-bit reduction (RED.E.ADD.F32x4) instead of four scalar atomics
-                                atomicAdd(reinterpret_cast<float4 *>(p + oy + (kx ? xhi : xlo) + oz), make_float4(w * gv.x, w * gv.y, w * gv.z, w * gv.w));
-                        }
-                    }
-                }
             }
+            float4 o = v[0];
+            if (DIM == 3) {
+                o.x = v[0].x + (v[1].x - v[0].x) * lz; o.y = v[0].y + (v[1].y - v[0].y) * lz;
+                o.z = v[0].z + (v[1].z - v[0].z) * lz; o.w = v[0].w + (v[1].w - v[0].w) * lz;
+            }
+            *(reinterpret_cast<float4 *>(dst + out_off) + c4) = o;
         }
         bl += dq; c4 += dr;
         if (c4 >= C4) { c4 -= C4; ++bl; }
     }
 }
 
-template <int DIM, bool BWD>
+template <int DIM>
 __global__ void __launch_bounds__(kRoiThreads) roi_cl4_per_roi(RoiGeom g, const float *__restrict__ src, const float *__restrict__ boxes,
                                                               const int *__restrict__ box_ind, float *__restrict__ dst, int bins_per_slice) {
     __shared__ RoiTables s;
-    roi_cl4_per_roi_body<DIM, BWD>(g, src, boxes, box_ind, dst, bins_per_slice, s);
+    roi_cl4_per_roi_body<DIM>(g, src, boxes, box_ind, dst, bins_per_slice, s);
 }
 
 // ---- pyramid variant: ONE launch for all levels of an FPN (replaces the per-level loop of models/mrcnn.py:405-447 — boolean-mask gather,
 // <= 4 crop_and_resize calls, concat, un-permute by sort).  Every RoI carries its level; its CTA reads that level's map geometry, so each
-// output row is written exactly once and, in the backward pass, each level's gradient map receives only its own RoIs.
+// output row is written exactly once.
 constexpr int kMaxPyrLevels = 5;
 struct PyrGeom {
     int num_boxes, batch, ch, cw, cz, C, nlevels;
     int64_t os[5];
     int H[kMaxPyrLevels], W[kMaxPyrLevels], Z[kMaxPyrLevels];
     int64_t is[kMaxPyrLevels][5];
-    float *map[kMaxPyrLevels];        // forward: source maps (read only); backward: gradient maps
+    float *map[kMaxPyrLevels];        // source maps (read only)
 };
 
-template <int DIM, bool BWD>
-__global__ void __launch_bounds__(kRoiThreads) roi_cl4_pyramid(const __grid_constant__ PyrGeom pg, const float *__restrict__ crops_or_grads,
-                                                              const float *__restrict__ boxes, const int *__restrict__ box_ind,
-                                                              const int *__restrict__ roi_level, float *__restrict__ crops_out, int bins_per_slice) {
+template <int DIM>
+__global__ void __launch_bounds__(kRoiThreads) roi_cl4_pyramid(const __grid_constant__ PyrGeom pg, const float *__restrict__ boxes,
+                                                              const int *__restrict__ box_ind, const int *__restrict__ roi_level,
+                                                              float *__restrict__ crops_out, int bins_per_slice) {
     __shared__ RoiTables s;
     int lv = roi_level[blockIdx.x];
     lv = lv < 0 ? 0 : (lv >= pg.nlevels ? pg.nlevels - 1 : lv);
@@ -334,8 +245,210 @@ __global__ void __launch_bounds__(kRoiThreads) roi_cl4_pyramid(const __grid_cons
     g.ch = pg.ch; g.cw = pg.cw; g.cz = pg.cz; g.C = pg.C;
 #pragma unroll
     for (int k = 0; k < 5; ++k) { g.is[k] = pg.is[lv][k]; g.os[k] = pg.os[k]; }
-    if (!BWD) roi_cl4_per_roi_body<DIM, false>(g, pg.map[lv], boxes, box_ind, crops_out, bins_per_slice, s);
-    else      roi_cl4_per_roi_body<DIM, true>(g, crops_or_grads, boxes, box_ind, pg.map[lv], bins_per_slice, s);
+    roi_cl4_per_roi_body<DIM>(g, pg.map[lv], boxes, box_ind, crops_out, bins_per_slice, s);
+}
+
+// ---------------------------------------------------------------- backward: a gather in a fixed order ----------------------------------------------------------------
+// Every element of the image gradient is owned by one thread, which adds the terms of every RoI sample that touches its voxel and writes the
+// element once: no atomics, no memset, no workspace, and two calls with the same arguments give the same bits.  One kernel serves all three
+// entry points (mdt_crop_and_resize_{2d,3d}_backward on any strides, mdt_pyramid_roi_align_backward over all levels at once); VEC = 4
+// moves 4 channels per item on channels-last maps and crops (the cl4_ok layouts), VEC = 1 one channel on any strides.  The arithmetic is
+// per channel and the same in both, so the result does not depend on the layout, the launch shape or the RoI chunking.
+//
+// Summation order (the definition of the result; tests/roi_gather_model.c restates it on the host):
+//   acc = 0 (zero_init = 1) or the element's prior content (zero_init = 0); then, for every RoI n in ascending index with box_ind[n] == the
+//   element's batch item (and, in the pyramid, clamped roi_level[n] == the map's level), for the bins and corners in lexicographic order of
+//   (oy, ky, ox, kx, oz, kz) — bin indices ascending, per axis the lo corner (ky = 0) before the hi corner — whose taps (sample_coord,
+//   make_tap: the forward's) equal the element's (y, x, z):
+//     w = wx * wz * wy (2D: wx * wy), each factor 1 - lerp (lo corner) or lerp (hi corner);  if w != 0: acc = acc + w * grad[n, c, oy, ox, oz]
+//   every product and sum rounded on its own (__fmul_rn / __fadd_rn: no contraction).  A zero weight skips the term, so an Inf or NaN
+//   gradient behind a zero-weight corner does not reach the element, as with the reference's `if (w != 0)`.
+//
+// A CTA owns a tile of TY x TX x TZ voxels times a slice of the channel groups of one (level, batch item).  It walks the RoIs in index order,
+// 256 at a time, and keeps (in order, by ballot) those of its item and level whose footprint meets the tile.  Footprint per axis: the taps of
+// the first and the last bin.  sample_coord is monotone in the bin index (every step - a product by a non-negative integer, a sum, a rounding,
+// a clamp - is monotone; the direction is that of hi - lo, so inverted boxes decrease), hence so are floor and ceil, and every bin's taps lie
+// between those of the end bins (tests/test_roi_gather_model_cpu.py).  The survivors are processed in groups of up to kGatherGroup: their tap
+// tables go to shared memory, then per (RoI, axis, tile coordinate) the first and last bin whose lo or hi tap is that coordinate, and each
+// thread walks those bin ranges for its items.  Bound: per element the work is the number of RoIs of its item and level that survive the
+// tile's cull plus the terms that touch it, which the scatter also executed (as one atomic each); the grads are read once per touching term.
+constexpr int kGatherItems = 4;       // (voxel, channel group) items per thread: the tile holds kRoiThreads * kGatherItems of them
+constexpr int kGatherGroup = 32;      // RoIs whose tap tables are staged at once
+constexpr int kGatherTapBudget = 2048;  // tap-table entries per group (24 KB): fewer RoIs per group once ch + cw + cz > 64
+constexpr int kTileBits = 10;         // local tile coordinates are packed y | x << 10 | z << 20
+constexpr int kMaxTileDim = 1 << kTileBits;
+
+struct GatherGeom {
+    int num_boxes, batch, ch, cw, cz, C, nlevels, zero_init, c_fastest;
+    int cs, ty, tx, tz, group;         // channel groups per CTA, tile extents, RoIs per tap-table group
+    int64_t os[5];
+    int H[kMaxPyrLevels], W[kMaxPyrLevels], Z[kMaxPyrLevels];
+    int nty[kMaxPyrLevels], ntx[kMaxPyrLevels], ntz[kMaxPyrLevels];
+    int cta_begin[kMaxPyrLevels + 1];  // first CTA (blockIdx.x) of each level; a level has batch * nty * ntx * ntz CTAs
+    int64_t is[kMaxPyrLevels][5];
+    float *map[kMaxPyrLevels];         // gradient maps
+};
+
+// does the footprint of the crop's taps on one axis meet the tile rows [t0, t0 + T)?
+__device__ __forceinline__ bool axis_meets_tile(float lo, float hi, int crop, int size, int t0, int T) {
+    const Tap a = make_tap(sample_coord(lo, hi, 0, crop, size)), b = make_tap(sample_coord(lo, hi, crop - 1, crop, size));
+    return max(a.hi, b.hi) >= t0 && min(a.lo, b.lo) < t0 + T;
+}
+
+template <int VEC> struct Vec;
+template <> struct Vec<1> {
+    static __device__ __forceinline__ void load(const float *p, float *v) { v[0] = __ldg(p); }
+    static __device__ __forceinline__ void load_rw(const float *p, float *v) { v[0] = *p; }
+    static __device__ __forceinline__ void store(float *p, const float *v) { *p = v[0]; }
+};
+template <> struct Vec<4> {
+    static __device__ __forceinline__ void load(const float *p, float *v) {
+        const float4 t = __ldg(reinterpret_cast<const float4 *>(p)); v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+    }
+    static __device__ __forceinline__ void load_rw(const float *p, float *v) {
+        const float4 t = *reinterpret_cast<const float4 *>(p); v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+    }
+    static __device__ __forceinline__ void store(float *p, const float *v) { *reinterpret_cast<float4 *>(p) = make_float4(v[0], v[1], v[2], v[3]); }
+};
+
+template <int DIM, int VEC>
+__global__ void __launch_bounds__(kRoiThreads) roi_bwd_gather(const __grid_constant__ GatherGeom g, const float *__restrict__ grads,
+                                                              const float *__restrict__ boxes, const int *__restrict__ box_ind,
+                                                              const int *__restrict__ roi_level) {
+    extern __shared__ __align__(16) unsigned char smem[];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int crop_sum = g.ch + g.cw + (DIM == 3 ? g.cz : 0), tile_sum = g.ty + g.tx + (DIM == 3 ? g.tz : 0);
+    int2 *rng = reinterpret_cast<int2 *>(smem);                                      // [group][tile_sum] bin range [x, y)
+    Tap *taps = reinterpret_cast<Tap *>(rng + g.group * tile_sum);                  // [group][crop_sum] y taps, x taps, z taps
+    int *surv = reinterpret_cast<int *>(taps + g.group * crop_sum);                 // [kRoiThreads] surviving RoIs of a chunk, in order
+    int *wcount = surv + kRoiThreads;                                               // [kRoiThreads / 32]
+
+    int lv = 0;
+    while (lv + 1 < g.nlevels && (int)blockIdx.x >= g.cta_begin[lv + 1]) ++lv;
+    int t = blockIdx.x - g.cta_begin[lv];
+    const int tzi = t % g.ntz[lv]; t /= g.ntz[lv];
+    const int txi = t % g.ntx[lv]; t /= g.ntx[lv];
+    const int tyi = t % g.nty[lv];
+    const int b = t / g.nty[lv];
+    const int y0 = tyi * g.ty, x0 = txi * g.tx, z0 = tzi * g.tz;
+    const int H = g.H[lv], W = g.W[lv], Z = g.Z[lv];
+    const int64_t *is = g.is[lv];
+    const int CG = g.C / VEC, cg0 = blockIdx.y * g.cs, ncs = min(g.cs, CG - cg0);
+    const int tv = g.ty * g.tx * g.tz;
+
+    // this thread's items: packed local voxel (-1: none / outside the map) and channel
+    int pos[kGatherItems], chan[kGatherItems];
+    float acc[kGatherItems][VEC];
+#pragma unroll
+    for (int k = 0; k < kGatherItems; ++k) {
+        const int item = tid + k * kRoiThreads;
+        int v, cg;
+        if (g.c_fastest) { v = item / ncs; cg = item - v * ncs; }
+        else             { cg = item / tv; v = item - cg * tv; }
+        const int lz = v % g.tz, lx = (v / g.tz) % g.tx, ly = v / (g.tz * g.tx);
+        const bool in = item < tv * ncs && y0 + ly < H && x0 + lx < W && z0 + lz < Z;
+        pos[k] = in ? (ly | (lx << kTileBits) | (lz << (2 * kTileBits))) : -1;
+        chan[k] = (cg0 + cg) * VEC;
+        float *p = g.map[lv] + b * is[0] + chan[k] * is[1] + (y0 + ly) * is[2] + (x0 + lx) * is[3] + (z0 + lz) * is[4];
+#pragma unroll
+        for (int i = 0; i < VEC; ++i) acc[k][i] = 0.f;
+        if (in && !g.zero_init) Vec<VEC>::load_rw(p, acc[k]);
+    }
+
+    for (int base = 0; base < g.num_boxes; base += kRoiThreads) {
+        const int n = base + tid;
+        bool keep = false;
+        if (n < g.num_boxes && box_ind[n] == b) {
+            int l = 0;
+            if (roi_level) { l = roi_level[n]; l = l < 0 ? 0 : (l >= g.nlevels ? g.nlevels - 1 : l); }
+            if (l == lv) {
+                const float *bx = boxes + (size_t)n * (2 * DIM);
+                keep = axis_meets_tile(bx[0], bx[2], g.ch, H, y0, g.ty) && axis_meets_tile(bx[1], bx[3], g.cw, W, x0, g.tx) &&
+                       (DIM == 2 || axis_meets_tile(bx[4], bx[5], g.cz, Z, z0, g.tz));
+            }
+        }
+        const unsigned ballot = __ballot_sync(0xffffffffu, keep);
+        if (lane == 0) wcount[warp] = __popc(ballot);
+        __syncthreads();
+        int before = 0, total = 0;
+#pragma unroll
+        for (int w = 0; w < kRoiThreads / 32; ++w) { before += w < warp ? wcount[w] : 0; total += wcount[w]; }
+        if (keep) surv[before + __popc(ballot & ((1u << lane) - 1u))] = n;
+        __syncthreads();
+
+        for (int r0 = 0; r0 < total; r0 += g.group) {
+            const int ng = min(g.group, total - r0);
+            for (int e = tid; e < ng * crop_sum; e += kRoiThreads) {
+                const int r = e / crop_sum, j = e - r * crop_sum;
+                const float *bx = boxes + (size_t)surv[r0 + r] * (2 * DIM);
+                if (j < g.ch)             taps[e] = make_tap(sample_coord(bx[0], bx[2], j, g.ch, H));
+                else if (j < g.ch + g.cw) taps[e] = make_tap(sample_coord(bx[1], bx[3], j - g.ch, g.cw, W));
+                else                      taps[e] = make_tap(sample_coord(bx[4], bx[5], j - g.ch - g.cw, g.cz, Z));
+            }
+            __syncthreads();
+            for (int e = tid; e < ng * tile_sum; e += kRoiThreads) {
+                const int r = e / tile_sum, j = e - r * tile_sum;
+                int v, first, crop;
+                if (j < g.ty)             { v = y0 + j;                first = 0;             crop = g.ch; }
+                else if (j < g.ty + g.tx) { v = x0 + j - g.ty;         first = g.ch;          crop = g.cw; }
+                else                      { v = z0 + j - g.ty - g.tx;  first = g.ch + g.cw;   crop = g.cz; }
+                const Tap *tp = taps + r * crop_sum + first;
+                int lo = crop, hi = 0;
+                for (int o = 0; o < crop; ++o)
+                    if (tp[o].lo == v || tp[o].hi == v) { lo = min(lo, o); hi = o + 1; }
+                rng[e] = make_int2(lo, hi);
+            }
+            __syncthreads();
+            for (int r = 0; r < ng; ++r) {
+                const Tap *ty_ = taps + r * crop_sum, *tx_ = ty_ + g.ch, *tz_ = tx_ + g.cw;
+                const int2 *rr = rng + r * tile_sum;
+                const float *gn = grads + (int64_t)surv[r0 + r] * g.os[0];
+#pragma unroll
+                for (int k = 0; k < kGatherItems; ++k) {
+                    if (pos[k] < 0) continue;
+                    const int ly = pos[k] & (kMaxTileDim - 1), lx = (pos[k] >> kTileBits) & (kMaxTileDim - 1), lz = pos[k] >> (2 * kTileBits);
+                    const int2 ry = rr[ly], rx = rr[g.ty + lx], rz = DIM == 3 ? rr[g.ty + g.tx + lz] : make_int2(0, 1);
+                    if (ry.x >= ry.y || rx.x >= rx.y || rz.x >= rz.y) continue;
+                    const int vy = y0 + ly, vx = x0 + lx, vz = z0 + lz;
+                    const float *gc = gn + chan[k] * g.os[1];
+                    for (int oy = ry.x; oy < ry.y; ++oy) {
+                        const Tap tyy = ty_[oy];
+                        for (int ky = 0; ky < 2; ++ky) {
+                            if ((ky ? tyy.hi : tyy.lo) != vy) continue;
+                            const float wy = ky ? tyy.lerp : 1 - tyy.lerp;
+                            for (int ox = rx.x; ox < rx.y; ++ox) {
+                                const Tap txx = tx_[ox];
+                                for (int kx = 0; kx < 2; ++kx) {
+                                    if ((kx ? txx.hi : txx.lo) != vx) continue;
+                                    const float wx = kx ? txx.lerp : 1 - txx.lerp;
+                                    for (int oz = rz.x; oz < rz.y; ++oz) {
+                                        const Tap tzz = DIM == 3 ? tz_[oz] : Tap{0, 0, 0.f};
+                                        for (int kz = 0; kz < (DIM == 3 ? 2 : 1); ++kz) {
+                                            if (DIM == 3 && (kz ? tzz.hi : tzz.lo) != vz) continue;
+                                            const float wz = kz ? tzz.lerp : 1 - tzz.lerp;
+                                            const float w = DIM == 3 ? __fmul_rn(__fmul_rn(wx, wz), wy) : __fmul_rn(wx, wy);
+                                            if (w == 0.f) continue;
+                                            float gv[VEC];
+                                            Vec<VEC>::load(gc + oy * g.os[2] + ox * g.os[3] + (DIM == 3 ? oz * g.os[4] : 0), gv);
+#pragma unroll
+                                            for (int i = 0; i < VEC; ++i) acc[k][i] = __fadd_rn(acc[k][i], __fmul_rn(w, gv[i]));
+                                        }
+                                    }
+                                }
+                            }
+                        }
+                    }
+                }
+            }
+            __syncthreads();
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < kGatherItems; ++k) {
+        if (pos[k] < 0) continue;
+        const int ly = pos[k] & (kMaxTileDim - 1), lx = (pos[k] >> kTileBits) & (kMaxTileDim - 1), lz = pos[k] >> (2 * kTileBits);
+        Vec<VEC>::store(g.map[lv] + b * is[0] + chan[k] * is[1] + (y0 + ly) * is[2] + (x0 + lx) * is[3] + (z0 + lz) * is[4], acc[k]);
+    }
 }
 
 // the per-RoI kernels keep tap offsets in 32 bits, tap tables of 64 entries per axis and <= 256 channel groups
@@ -385,7 +498,7 @@ static int roi_forward(const float *image, const int64_t *is, const float *boxes
     if (cl4_ok(g, image, crops) && per_roi_ok(g)) {
         dim3 grid; int bins;
         per_roi_grid(g, grid, bins);
-        roi_cl4_per_roi<DIM, false><<<grid, kRoiThreads, 0, st>>>(g, image, boxes, box_ind, crops, bins);
+        roi_cl4_per_roi<DIM><<<grid, kRoiThreads, 0, st>>>(g, image, boxes, box_ind, crops, bins);
     } else if (cl4_ok(g, image, crops)) {
         if (small) roi_fwd_cl4<DIM, unsigned><<<grid_for(total / 4, 256), 256, 0, st>>>(g, image, boxes, box_ind, crops, total / 4);
         else       roi_fwd_cl4<DIM, long long><<<grid_for(total / 4, 256), 256, 0, st>>>(g, image, boxes, box_ind, crops, total / 4);
@@ -397,34 +510,62 @@ static int roi_forward(const float *image, const int64_t *is, const float *boxes
     return launch_status();
 }
 
+// Launches roi_bwd_gather over the levels already in g (nlevels, H/W/Z, is, map), after the tile and grid geometry are derived here.
+template <int DIM>
+static int gather_launch(GatherGeom &g, bool vec, const float *grads, const float *boxes, const int *box_ind, const int *roi_level, cudaStream_t st) {
+    const int CG = vec ? g.C / 4 : g.C;
+    const int slices = ceil_div(CG, kRoiThreads);
+    g.cs = ceil_div(CG, slices);
+    // tile: powers of two per axis (z, x, y in turn) up to the largest level's extent, as many voxels as kGatherItems items per thread allow
+    const int tv_max = kRoiThreads * kGatherItems / g.cs;
+    int Hm = 1, Wm = 1, Zm = 1;
+    for (int l = 0; l < g.nlevels; ++l) { Hm = std::max(Hm, g.H[l]); Wm = std::max(Wm, g.W[l]); Zm = std::max(Zm, g.Z[l]); }
+    g.ty = g.tx = g.tz = 1;
+    for (bool grown = true; grown;) {
+        grown = false;
+        int *t[3] = {&g.tz, &g.tx, &g.ty};
+        const int ext[3] = {DIM == 3 ? Zm : 1, Wm, Hm};
+        for (int a = 0; a < 3; ++a)
+            if (g.ty * g.tx * g.tz * 2 <= tv_max && *t[a] < ext[a] && *t[a] < kMaxTileDim / 2) { *t[a] *= 2; grown = true; }
+    }
+    long long ctas = 0;
+    for (int l = 0; l < g.nlevels; ++l) {
+        g.nty[l] = ceil_div(g.H[l], g.ty); g.ntx[l] = ceil_div(g.W[l], g.tx); g.ntz[l] = ceil_div(g.Z[l], g.tz);
+        g.cta_begin[l] = (int)ctas;
+        ctas += (long long)g.batch * g.nty[l] * g.ntx[l] * g.ntz[l];
+        if (ctas >= (1LL << 31)) return MDT_EUNSUPPORTED;
+    }
+    g.cta_begin[g.nlevels] = (int)ctas;
+    const int crop_sum = g.ch + g.cw + (DIM == 3 ? g.cz : 0), tile_sum = g.ty + g.tx + (DIM == 3 ? g.tz : 0);
+    g.group = std::max(1, std::min(kGatherGroup, kGatherTapBudget / crop_sum));
+    const size_t smem = (size_t)g.group * tile_sum * sizeof(int2) + (size_t)g.group * crop_sum * sizeof(Tap) + (kRoiThreads + kRoiThreads / 32) * sizeof(int);
+    auto kernel = vec ? roi_bwd_gather<DIM, 4> : roi_bwd_gather<DIM, 1>;
+    if (smem > 48 * 1024) {   // very large crops only: one RoI's tap tables at a time, past the default shared-memory window
+        int dev = 0, optin = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
+            smem > (size_t)optin)
+            return MDT_EUNSUPPORTED;
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return (int)e;
+    }
+    kernel<<<dim3((unsigned)ctas, (unsigned)slices, 1), kRoiThreads, smem, st>>>(g, grads, boxes, box_ind, roi_level);
+    return launch_status();
+}
+
 template <int DIM>
 static int roi_backward(const float *grads, const int64_t *gs, const float *boxes, const int *box_ind, int num_boxes, int batch, int H, int W, int Z,
                         int ch, int cw, int cz, int C, float *gimg, const int64_t *is, int zero_init, int64_t image_numel, cudaStream_t st) {
     if (num_boxes < 0 || batch <= 0 || H <= 0 || W <= 0 || Z <= 0 || ch <= 0 || cw <= 0 || cz <= 0 || C <= 0 || !is || !gs || !gimg) return MDT_EINVAL;
-    if (zero_init) {
-        if (image_numel <= 0) return MDT_EINVAL;
-        cudaError_t e = cudaMemsetAsync(gimg, 0, (size_t)image_numel * sizeof(float), st);
-        if (e != cudaSuccess) return (int)e;
-    }
-    if (num_boxes == 0) return MDT_OK;
-    if (!grads || !boxes || !box_ind) return MDT_EINVAL;
-    RoiGeom g{num_boxes, batch, H, W, Z, ch, cw, cz, C, {0, 0, 0, 0, 0}, {0, 0, 0, 0, 0}};
-    for (int k = 0; k < DIM + 2; ++k) { g.is[k] = is[k]; g.os[k] = gs[k]; }
-    const long long total = (long long)num_boxes * C * ch * cw * cz;
-    const bool small = fits_u32(total);
-    if (cl4_ok(g, gimg, grads) && per_roi_ok(g)) {
-        dim3 grid; int bins;
-        per_roi_grid(g, grid, bins);
-        roi_cl4_per_roi<DIM, true><<<grid, kRoiThreads, 0, st>>>(g, grads, boxes, box_ind, gimg, bins);
-    } else if (cl4_ok(g, gimg, grads)) {
-        if (small) roi_bwd_cl4<DIM, unsigned><<<grid_for(total / 4, 256), 256, 0, st>>>(g, grads, boxes, box_ind, gimg, total / 4);
-        else       roi_bwd_cl4<DIM, long long><<<grid_for(total / 4, 256), 256, 0, st>>>(g, grads, boxes, box_ind, gimg, total / 4);
-    } else {
-        const int c_fastest = (g.is[1] == 1);
-        if (small) roi_bwd_scalar<DIM, unsigned><<<grid_for(total, 256), 256, 0, st>>>(g, grads, boxes, box_ind, gimg, c_fastest, total);
-        else       roi_bwd_scalar<DIM, long long><<<grid_for(total, 256), 256, 0, st>>>(g, grads, boxes, box_ind, gimg, c_fastest, total);
-    }
-    return launch_status();
+    if (zero_init && image_numel <= 0) return MDT_EINVAL;
+    if (num_boxes == 0 && !zero_init) return MDT_OK;
+    if (num_boxes > 0 && (!grads || !boxes || !box_ind)) return MDT_EINVAL;
+    RoiGeom rg{num_boxes, batch, H, W, Z, ch, cw, cz, C, {0, 0, 0, 0, 0}, {0, 0, 0, 0, 0}};
+    GatherGeom g{};
+    g.num_boxes = num_boxes; g.batch = batch; g.ch = ch; g.cw = cw; g.cz = cz; g.C = C; g.nlevels = 1; g.zero_init = zero_init != 0;
+    g.H[0] = H; g.W[0] = W; g.Z[0] = Z; g.map[0] = gimg;
+    for (int k = 0; k < DIM + 2; ++k) { rg.is[k] = g.is[0][k] = is[k]; rg.os[k] = g.os[k] = gs[k]; }
+    g.c_fastest = is[1] == 1;
+    return gather_launch<DIM>(g, cl4_ok(rg, gimg, grads), grads, boxes, box_ind, nullptr, st);
 }
 
 template <int DIM>
@@ -445,19 +586,25 @@ static int pyramid_run(bool bwd, float *const *maps, const int64_t *is, const in
         RoiGeom g{num_boxes, batch, pg.H[l], pg.W[l], pg.Z[l], ch, cw, cz, C, {0, 0, 0, 0, 0}, {0, 0, 0, 0, 0}};
         for (int k = 0; k < 5; ++k) { g.is[k] = pg.is[l][k]; g.os[k] = pg.os[k]; }
         if (!cl4_ok(g, maps[l], crop_ptr) || !per_roi_ok(g)) return MDT_EUNSUPPORTED;   // caller falls back to one launch per level
-        if (bwd && zero_init) {
-            if (!numel || numel[l] <= 0) return MDT_EINVAL;
-            cudaError_t e = cudaMemsetAsync(maps[l], 0, (size_t)numel[l] * sizeof(float), st);
-            if (e != cudaSuccess) return (int)e;
-        }
+        if (bwd && zero_init && (!numel || numel[l] <= 0)) return MDT_EINVAL;
     }
-    if (num_boxes == 0) return MDT_OK;
-    if (!boxes || !box_ind || !roi_level || !crop_ptr) return MDT_EINVAL;
+    if (num_boxes == 0 && !(bwd && zero_init)) return MDT_OK;
+    if (num_boxes > 0 && (!boxes || !box_ind || !roi_level || !crop_ptr)) return MDT_EINVAL;
+    if (bwd) {
+        GatherGeom g{};
+        g.num_boxes = num_boxes; g.batch = batch; g.ch = ch; g.cw = cw; g.cz = cz; g.C = C; g.nlevels = nlevels; g.zero_init = zero_init != 0;
+        g.c_fastest = 1;
+        for (int k = 0; k < 5; ++k) g.os[k] = pg.os[k];
+        for (int l = 0; l < nlevels; ++l) {
+            g.H[l] = pg.H[l]; g.W[l] = pg.W[l]; g.Z[l] = pg.Z[l]; g.map[l] = pg.map[l];
+            for (int k = 0; k < 5; ++k) g.is[l][k] = pg.is[l][k];
+        }
+        return gather_launch<DIM>(g, true, crops_or_grads, boxes, box_ind, roi_level, st);
+    }
     RoiGeom g0{num_boxes, batch, pg.H[0], pg.W[0], pg.Z[0], ch, cw, cz, C, {0, 0, 0, 0, 0}, {0, 0, 0, 0, 0}};
     dim3 grid; int bins;
     per_roi_grid(g0, grid, bins);
-    if (!bwd) roi_cl4_pyramid<DIM, false><<<grid, kRoiThreads, 0, st>>>(pg, nullptr, boxes, box_ind, roi_level, crops_out, bins);
-    else      roi_cl4_pyramid<DIM, true><<<grid, kRoiThreads, 0, st>>>(pg, crops_or_grads, boxes, box_ind, roi_level, nullptr, bins);
+    roi_cl4_pyramid<DIM><<<grid, kRoiThreads, 0, st>>>(pg, boxes, box_ind, roi_level, crops_out, bins);
     return launch_status();
 }
 

@@ -6,7 +6,7 @@ load key-for-key).
   -------------------------------------------------------  -----------------------------------------------------------------------
   RPN / Classifier / Mask heads           mrcnn.py:40-169  same modules on tensor-core convs; ConvTranspose3d(k2,s2) = 1x1x1 conv + voxel shuffle
   proposal_layer (sort, NMS 0.7, pad)     :297-369         top-k + csrc/nms.cu with on-device reduction; fixed-shape padding, NO host sync
-  pyramid_roi_align                       :373-457         csrc/roi_align.cu (channels-last, 128-bit gathers / vector atomics in backward)
+  pyramid_roi_align                       :373-457         csrc/roi_align.cu (channels-last, 128-bit gathers; fixed-order gather backward)
   detection_target_layer                  :461-613         broadcast IoU, RoIAlign on GT masks, device SHEM
   refine_detections                       :620-714         one batched multi-class NMS launch (groups translated apart), top-k per element
   numpy gt_anchor_matching per element    :894             fp64 device kernels (csrc/anchor_match.cu) on a side stream
