@@ -182,6 +182,12 @@ int mdt_conv3d_variant(const mdt_conv3d_desc *desc_host, int pass);
  * adjoint, written as a gather (no atomics, no zero fill). */
 int mdt_upsample221_forward(const float *x, float *y, int n, int d, int h, int w, int c, void *stream);
 int mdt_upsample221_backward(const float *gy, float *gx, int n, int d, int h, int w, int c, void *stream);
+/* The same (2,2,1) map and gather adjoint for any c >= 1 and fp32 pointers aligned to 4 bytes (else MDT_EINVAL), accessing V = 4, 2 or 1
+ * channels at a time as the pooling kernels below do.  Also replaces F.interpolate(x, scale_factor=2, mode='bilinear', align_corners=False) of
+ * the 2D decoder: an NHWC map is passed with w = 1.  Each element's arithmetic and its order of the 16 gather terms do not depend on V: the
+ * result equals mdt_upsample221_* bit for bit where both accept the arguments, and the backward is bit-reproducible. */
+int mdt_upsample_linear2x_forward(const float *x, float *y, int n, int d, int h, int w, int c, void *stream);
+int mdt_upsample_linear2x_backward(const float *gy, float *gx, int n, int d, int h, int w, int c, void *stream);
 
 /* ------------------------------------------------------------- pooling / nearest up-sampling -------------------------------------------------
  * replaces: nn.MaxPool3d(kernel_size=3, stride=(2,2,1), padding=1) / nn.MaxPool2d(3, 2, 1) of models/backbone.py:63-64 (applied at :129) and its

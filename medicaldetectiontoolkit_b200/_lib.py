@@ -75,6 +75,8 @@ SIGNATURES = {
     "mdt_conv3d_fprop_out": (_I, [ctypes.POINTER(Conv3dDesc), _VP, _VP, _VP, _VP, _VP, _VP, _VP, _SZ, _VP]),
     "mdt_upsample221_forward": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _VP]),
     "mdt_upsample221_backward": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _VP]),
+    "mdt_upsample_linear2x_forward": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _VP]),
+    "mdt_upsample_linear2x_backward": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _VP]),
     "mdt_maxpool3d_forward": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _I, ctypes.POINTER(_I), ctypes.POINTER(_I), ctypes.POINTER(_I), _VP]),
     "mdt_maxpool3d_backward": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _I, ctypes.POINTER(_I), ctypes.POINTER(_I), ctypes.POINTER(_I), _VP]),
     "mdt_upsample_nearest_forward": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _VP]),

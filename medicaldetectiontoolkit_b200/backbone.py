@@ -76,17 +76,20 @@ class ResBlock(nn.Module):
 
 
 class _Upsample221(torch.autograd.Function):
-    """(2,2,1) trilinear up-sampling of a channels-last map on libmdt_b200 (csrc/resample.cu); backward = gather adjoint"""
+    """(2,2,1) trilinear up-sampling of a channels-last map on libmdt_b200 (csrc/resample.cu); backward = gather adjoint.  any_c selects
+    mdt_upsample_linear2x_* (any channel count, V = 4 / 2 / 1 channels per access) instead of the float4-only mdt_upsample221_*"""
 
     @staticmethod
-    def forward(ctx, x):
+    def forward(ctx, x, any_c=False):
         lib = L.load()
         x = _cl3_aligned(x)
         n, c, d, h, w = x.shape
         y = torch.empty((n, c, 2 * d, 2 * h, w), dtype=x.dtype, device=x.device, memory_format=_CL3)
+        fwd = lib.mdt_upsample_linear2x_forward if any_c else lib.mdt_upsample221_forward
         with torch.cuda.device(x.device):
-            L.check(lib.mdt_upsample221_forward(L.ptr(x), L.ptr(y), n, d, h, w, c, L.stream_ptr()))
+            L.check(fwd(L.ptr(x), L.ptr(y), n, d, h, w, c, L.stream_ptr()))
         ctx.shape = (n, c, d, h, w)
+        ctx.any_c = any_c
         return y
 
     @staticmethod
@@ -95,14 +98,16 @@ class _Upsample221(torch.autograd.Function):
         n, c, d, h, w = ctx.shape
         gy = _cl3_aligned(gy)
         gx = torch.empty((n, c, d, h, w), dtype=gy.dtype, device=gy.device, memory_format=_CL3)
+        bwd = lib.mdt_upsample_linear2x_backward if ctx.any_c else lib.mdt_upsample221_backward
         with torch.cuda.device(gy.device):
-            L.check(lib.mdt_upsample221_backward(L.ptr(gy), L.ptr(gx), n, d, h, w, c, L.stream_ptr()))
-        return gx
+            L.check(bwd(L.ptr(gy), L.ptr(gx), n, d, h, w, c, L.stream_ptr()))
+        return gx, None
 
 
 def _cl3_aligned(t):
     """t as a channels-last-3d tensor whose data pointer is 16-byte aligned: .contiguous() keeps the storage offset of an already-contiguous
-    view, and the float4 paths of csrc/resample.cu refuse a misaligned base (MDT_EINVAL), so such a view is copied"""
+    view, and the float4 paths of csrc/resample.cu refuse a misaligned base (MDT_EINVAL) while the others fall back to narrower accesses, so
+    such a view is copied"""
     t = t.contiguous(memory_format=_CL3)
     return t if t.data_ptr() % 16 == 0 else t.clone(memory_format=_CL3)
 
@@ -202,9 +207,14 @@ class Interpolate(nn.Module):
         self.mode = mode
 
     def forward(self, x):
-        if (x.is_cuda and x.dim() == 5 and x.dtype == torch.float32 and self.mode == 'trilinear' and tuple(self.scale_factor) == (2, 2, 1)
-                and x.shape[1] % 4 == 0):
-            return _Upsample221.apply(x)
+        """CUDA fp32 maps run on the library: 5-D trilinear (2,2,1) (float4 kernels at C % 4 == 0, any C otherwise) and 4-D bilinear x2 as
+        the same map of x.unsqueeze(-1) (channels-last-3d with w = 1); both backwards are fixed-order gathers"""
+        if x.is_cuda and x.dtype == torch.float32:
+            sf = tuple(self.scale_factor) if isinstance(self.scale_factor, (tuple, list)) else (self.scale_factor,) * (x.dim() - 2)
+            if x.dim() == 5 and self.mode == 'trilinear' and sf == (2, 2, 1):
+                return _Upsample221.apply(x, x.shape[1] % 4 != 0)
+            if x.dim() == 4 and self.mode == 'bilinear' and sf == (2, 2):
+                return _Upsample221.apply(x.unsqueeze(-1), True).squeeze(-1)
         return F.interpolate(x, scale_factor=self.scale_factor, mode=self.mode, align_corners=False)
 
 

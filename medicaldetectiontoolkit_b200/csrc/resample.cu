@@ -1,86 +1,16 @@
 // (2,2,1) trilinear up-sampling (align_corners = False) for NDHWC maps — the P2->P1->P0 decoder steps of the full-resolution FPN path
-// (models/backbone.py:172-173 `Interpolate(scale_factor=(2,2,1), mode='trilinear')`, executed by F.interpolate in the reference).
+// (models/backbone.py:172-173 `Interpolate(scale_factor=(2,2,1), mode='trilinear')`, executed by F.interpolate in the reference).  2D bilinear x2
+// (`Interpolate(scale_factor=2, mode='bilinear')`) is the same map on an NHWC tensor viewed as NDHWC with w = 1.
 // With scale 2 and half-pixel centres the interpolation weights are the constants 0.25 / 0.75 along y and x (z is copied), edges clamp:
 //   out[2i] = 0.25 x[max(i-1,0)] + 0.75 x[i],   out[2i+1] = 0.75 x[i] + 0.25 x[min(i+1, n-1)]
-// Forward is a pure streaming kernel (float4 over channels); backward is written as a GATHER (each input voxel sums its <= 16
-// contributing output gradients), so it needs no atomics and no zero-fill — the library's scatter version spends 4.4 ms on a
-// [2,36,128,128,128] map, this one is bandwidth-bound.
+// Forward is a pure streaming kernel; backward is written as a GATHER (each input voxel sums its 16 contributing output gradients in a fixed
+// order), so it needs no atomics and no zero-fill and is bit-reproducible — the library's scatter version spent 4.4 ms on a [2,36,128,128,128]
+// map, this one is bandwidth-bound.  Both access V = 4, 2 or 1 channels at a time (vec_of below); every product and sum is an explicit
+// __fmul_rn / __fmaf_rn in the shape nvcc gave the earlier float4-only kernels, so an element's bits do not depend on V and V = 4 keeps them.
 #include "mdt_common.cuh"
 
 namespace mdt {
 
-__device__ __forceinline__ void up_taps(int o, int n, int &i0, int &i1, float &w0, float &w1) {
-    const int i = o >> 1;
-    if (o & 1) { i0 = i; i1 = min(i + 1, n - 1); w0 = 0.75f; w1 = 0.25f; }
-    else       { i0 = max(i - 1, 0); i1 = i; w0 = 0.25f; w1 = 0.75f; }
-}
-
-// x [N, D, H, W, C] -> y [N, 2D, 2H, W, C]; one thread = one output voxel x 4 channels
-__global__ void __launch_bounds__(256) upsample221_fwd_kernel(const float *__restrict__ x, float *__restrict__ y, int N, int D, int H, int W, int C4) {
-    const long long total = (long long)N * 2 * D * 2 * H * W * C4;
-    const float4 *x4 = reinterpret_cast<const float4 *>(x);
-    float4 *y4 = reinterpret_cast<float4 *>(y);
-    for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
-        long long r = t;
-        const int c = r % C4; r /= C4;
-        const int w = r % W; r /= W;
-        const int oh = r % (2 * H); r /= 2 * H;
-        const int od = r % (2 * D);
-        const int n = (int)(r / (2 * D));
-        int d0, d1, h0, h1; float wd0, wd1, wh0, wh1;
-        up_taps(od, D, d0, d1, wd0, wd1);
-        up_taps(oh, H, h0, h1, wh0, wh1);
-        auto at = [&](int d, int h) { return __ldg(x4 + ((((long long)n * D + d) * H + h) * W + w) * C4 + c); };
-        const float4 a = at(d0, h0), b = at(d0, h1), e = at(d1, h0), f = at(d1, h1);
-        float4 o;
-        o.x = wd0 * (wh0 * a.x + wh1 * b.x) + wd1 * (wh0 * e.x + wh1 * f.x);
-        o.y = wd0 * (wh0 * a.y + wh1 * b.y) + wd1 * (wh0 * e.y + wh1 * f.y);
-        o.z = wd0 * (wh0 * a.z + wh1 * b.z) + wd1 * (wh0 * e.z + wh1 * f.z);
-        o.w = wd0 * (wh0 * a.w + wh1 * b.w) + wd1 * (wh0 * e.w + wh1 * f.w);
-        y4[t] = o;
-    }
-}
-
-// 1-D adjoint taps of input index i: output indices and weights (edge clamping folds the out-of-range neighbour onto the border output)
-__device__ __forceinline__ int down_taps(int i, int n, int *o, float *w) {
-    int k = 0;
-    o[k] = 2 * i; w[k++] = 0.75f;
-    o[k] = 2 * i + 1; w[k++] = 0.75f;
-    if (i > 0) { o[k] = 2 * i - 1; w[k++] = 0.25f; } else { o[k] = 0; w[k++] = 0.25f; }
-    if (i < n - 1) { o[k] = 2 * i + 2; w[k++] = 0.25f; } else { o[k] = 2 * n - 1; w[k++] = 0.25f; }
-    return k;
-}
-
-__global__ void __launch_bounds__(256) upsample221_bwd_kernel(const float *__restrict__ gy, float *__restrict__ gx, int N, int D, int H, int W, int C4) {
-    const long long total = (long long)N * D * H * W * C4;
-    const float4 *g4 = reinterpret_cast<const float4 *>(gy);
-    float4 *o4 = reinterpret_cast<float4 *>(gx);
-    for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
-        long long r = t;
-        const int c = r % C4; r /= C4;
-        const int w = r % W; r /= W;
-        const int h = r % H; r /= H;
-        const int d = r % D;
-        const int n = (int)(r / D);
-        int od[4], oh[4]; float wd[4], wh[4];
-        const int nd = down_taps(d, D, od, wd), nh = down_taps(h, H, oh, wh);
-        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-        for (int a = 0; a < nd; ++a)
-            for (int b = 0; b < nh; ++b) {
-                const float4 v = __ldg(g4 + ((((long long)n * 2 * D + od[a]) * 2 * H + oh[b]) * W + w) * C4 + c);
-                const float ww = wd[a] * wh[b];
-                acc.x += ww * v.x; acc.y += ww * v.y; acc.z += ww * v.z; acc.w += ww * v.w;
-            }
-        o4[t] = acc;
-    }
-}
-
-
-// ------------------------------------------------------------------------------------------------ max pooling
-// nn.MaxPool3d(kernel_size=3, stride=(2,2,1), padding=1) / nn.MaxPool2d(3, 2, 1) in front of C2 (models/backbone.py:63-64, used at :129) for
-// NDHWC maps.  Forward: one thread = one output voxel x V channels, window scanned in (d, h, w) order with ATen's update rule
-// (`val > max || isnan(val)`: first maximum wins, NaN propagates) and the winning window offset kept as one byte per element.  Backward is a
-// GATHER over the <= 2 x 2 x 3 windows that contain an input voxel (no atomics, no zero fill): the gradient goes to the arg-max element only.
 template <int V> struct VecT;
 template <> struct VecT<4> { using type = float4; };
 template <> struct VecT<2> { using type = float2; };
@@ -102,6 +32,89 @@ __device__ __forceinline__ void st_vec(float *p, const float (&v)[V]) {
     *reinterpret_cast<typename VecT<V>::type *>(p) = t;
 }
 
+__device__ __forceinline__ void up_taps(int o, int n, int &i0, int &i1, float &w0, float &w1) {
+    const int i = o >> 1;
+    if (o & 1) { i0 = i; i1 = min(i + 1, n - 1); w0 = 0.75f; w1 = 0.25f; }
+    else       { i0 = max(i - 1, 0); i1 = i; w0 = 0.25f; w1 = 0.75f; }
+}
+
+// x [N, D, H, W, C] -> y [N, 2D, 2H, W, C]; one thread = one output voxel x V channels
+template <int V>
+__global__ void __launch_bounds__(256) upsample221_fwd_kernel(const float *__restrict__ x, float *__restrict__ y, int N, int D, int H, int W, int C) {
+    const int CV = C / V;
+    const long long total = (long long)N * 2 * D * 2 * H * W * CV;
+    for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
+        long long r = t;
+        const int c = (int)(r % CV) * V; r /= CV;
+        const int w = r % W; r /= W;
+        const int oh = r % (2 * H); r /= 2 * H;
+        const int od = r % (2 * D);
+        const int n = (int)(r / (2 * D));
+        int d0, d1, h0, h1; float wd0, wd1, wh0, wh1;
+        up_taps(od, D, d0, d1, wd0, wd1);
+        up_taps(oh, H, h0, h1, wh0, wh1);
+        auto at = [&](int d, int h) { return x + ((((long long)n * D + d) * H + h) * W + w) * C + c; };
+        float a[V], b[V], e[V], f[V], o[V];
+        ld_vec<V>(at(d0, h0), a);
+        ld_vec<V>(at(d0, h1), b);
+        ld_vec<V>(at(d1, h0), e);
+        ld_vec<V>(at(d1, h1), f);
+#pragma unroll
+        for (int i = 0; i < V; ++i) {
+            // wd0 * (wh0 * a + wh1 * b) + wd1 * (wh0 * e + wh1 * f), contracted as nvcc contracts it in the float4 kernel
+            const float lo = __fmaf_rn(wh0, a[i], __fmul_rn(wh1, b[i]));
+            const float hi = __fmaf_rn(wh0, e[i], __fmul_rn(wh1, f[i]));
+            o[i] = __fmaf_rn(wd0, lo, __fmul_rn(wd1, hi));
+        }
+        st_vec<V>(y + t * V, o);
+    }
+}
+
+// 1-D adjoint taps of input index i: output indices and weights (edge clamping folds the out-of-range neighbour onto the border output)
+__device__ __forceinline__ int down_taps(int i, int n, int *o, float *w) {
+    int k = 0;
+    o[k] = 2 * i; w[k++] = 0.75f;
+    o[k] = 2 * i + 1; w[k++] = 0.75f;
+    if (i > 0) { o[k] = 2 * i - 1; w[k++] = 0.25f; } else { o[k] = 0; w[k++] = 0.25f; }
+    if (i < n - 1) { o[k] = 2 * i + 2; w[k++] = 0.25f; } else { o[k] = 2 * n - 1; w[k++] = 0.25f; }
+    return k;
+}
+
+// gx [N, D, H, W, C] from gy [N, 2D, 2H, W, C]: acc = fma(wd * wh, gy, acc) from +0 over the (d, h) taps in down_taps order; wd * wh is exact
+template <int V>
+__global__ void __launch_bounds__(256) upsample221_bwd_kernel(const float *__restrict__ gy, float *__restrict__ gx, int N, int D, int H, int W, int C) {
+    const int CV = C / V;
+    const long long total = (long long)N * D * H * W * CV;
+    for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
+        long long r = t;
+        const int c = (int)(r % CV) * V; r /= CV;
+        const int w = r % W; r /= W;
+        const int h = r % H; r /= H;
+        const int d = r % D;
+        const int n = (int)(r / D);
+        int od[4], oh[4]; float wd[4], wh[4];
+        const int nd = down_taps(d, D, od, wd), nh = down_taps(h, H, oh, wh);
+        float acc[V];
+#pragma unroll
+        for (int i = 0; i < V; ++i) acc[i] = 0.f;
+        for (int a = 0; a < nd; ++a)
+            for (int b = 0; b < nh; ++b) {
+                float v[V];
+                ld_vec<V>(gy + ((((long long)n * 2 * D + od[a]) * 2 * H + oh[b]) * W + w) * C + c, v);
+                const float ww = __fmul_rn(wd[a], wh[b]);
+#pragma unroll
+                for (int i = 0; i < V; ++i) acc[i] = __fmaf_rn(ww, v[i], acc[i]);
+            }
+        st_vec<V>(gx + t * V, acc);
+    }
+}
+
+
+// ------------------------------------------------------------------------------------------------ max pooling
+// nn.MaxPool3d(kernel_size=3, stride=(2,2,1), padding=1) / nn.MaxPool2d(3, 2, 1) in front of C2 (models/backbone.py:63-64, used at :129) for
+// NDHWC maps.  Forward: one thread = one output voxel x V channels, window scanned in (d, h, w) order with ATen's update rule
+// (`val > max || isnan(val)`: first maximum wins, NaN propagates) and the winning window offset kept as one byte per element.  Backward is a
+// GATHER over the <= 2 x 2 x 3 windows that contain an input voxel (no atomics, no zero fill): the gradient goes to the arg-max element only.
 struct PoolGeom { int N, D, H, W, C, OD, OH, OW, kd, kh, kw, sd, sh, sw, pd, ph, pw; };
 
 template <int V>
@@ -245,19 +258,39 @@ extern "C" {
 
 int mdt_upsample221_forward(const float *x, float *y, int n, int d, int h, int w, int c, void *stream) {
     if (!x || !y || n <= 0 || d <= 0 || h <= 0 || w <= 0 || c <= 0 || c % 4 || !mdt::aligned(x, 16) || !mdt::aligned(y, 16)) return MDT_EINVAL;
-    const long long total = (long long)n * 2 * d * 2 * h * w * (c / 4);
-    long long blocks = mdt::ceil_div<long long>(total, 256);
-    if (blocks > (long long)mdt::num_sms() * 32) blocks = (long long)mdt::num_sms() * 32;
-    mdt::upsample221_fwd_kernel<<<(unsigned)blocks, 256, 0, mdt::as_stream(stream)>>>(x, y, n, d, h, w, c / 4);
+    const unsigned blocks = mdt::stream_blocks((long long)n * 2 * d * 2 * h * w * (c / 4));
+    mdt::upsample221_fwd_kernel<4><<<blocks, 256, 0, mdt::as_stream(stream)>>>(x, y, n, d, h, w, c);
     return mdt::launch_status();
 }
 
 int mdt_upsample221_backward(const float *gy, float *gx, int n, int d, int h, int w, int c, void *stream) {
     if (!gy || !gx || n <= 0 || d <= 0 || h <= 0 || w <= 0 || c <= 0 || c % 4 || !mdt::aligned(gy, 16) || !mdt::aligned(gx, 16)) return MDT_EINVAL;
-    const long long total = (long long)n * d * h * w * (c / 4);
-    long long blocks = mdt::ceil_div<long long>(total, 256);
-    if (blocks > (long long)mdt::num_sms() * 32) blocks = (long long)mdt::num_sms() * 32;
-    mdt::upsample221_bwd_kernel<<<(unsigned)blocks, 256, 0, mdt::as_stream(stream)>>>(gy, gx, n, d, h, w, c / 4);
+    const unsigned blocks = mdt::stream_blocks((long long)n * d * h * w * (c / 4));
+    mdt::upsample221_bwd_kernel<4><<<blocks, 256, 0, mdt::as_stream(stream)>>>(gy, gx, n, d, h, w, c);
+    return mdt::launch_status();
+}
+
+int mdt_upsample_linear2x_forward(const float *x, float *y, int n, int d, int h, int w, int c, void *stream) {
+    if (!x || !y || n <= 0 || d <= 0 || h <= 0 || w <= 0 || c <= 0) return MDT_EINVAL;
+    const int v = mdt::vec_of(c, x, y);
+    if (!v) return MDT_EINVAL;
+    const unsigned blocks = mdt::stream_blocks((long long)n * 2 * d * 2 * h * w * (c / v));
+    cudaStream_t st = mdt::as_stream(stream);
+    if (v == 4) mdt::upsample221_fwd_kernel<4><<<blocks, 256, 0, st>>>(x, y, n, d, h, w, c);
+    else if (v == 2) mdt::upsample221_fwd_kernel<2><<<blocks, 256, 0, st>>>(x, y, n, d, h, w, c);
+    else mdt::upsample221_fwd_kernel<1><<<blocks, 256, 0, st>>>(x, y, n, d, h, w, c);
+    return mdt::launch_status();
+}
+
+int mdt_upsample_linear2x_backward(const float *gy, float *gx, int n, int d, int h, int w, int c, void *stream) {
+    if (!gy || !gx || n <= 0 || d <= 0 || h <= 0 || w <= 0 || c <= 0) return MDT_EINVAL;
+    const int v = mdt::vec_of(c, gy, gx);
+    if (!v) return MDT_EINVAL;
+    const unsigned blocks = mdt::stream_blocks((long long)n * d * h * w * (c / v));
+    cudaStream_t st = mdt::as_stream(stream);
+    if (v == 4) mdt::upsample221_bwd_kernel<4><<<blocks, 256, 0, st>>>(gy, gx, n, d, h, w, c);
+    else if (v == 2) mdt::upsample221_bwd_kernel<2><<<blocks, 256, 0, st>>>(gy, gx, n, d, h, w, c);
+    else mdt::upsample221_bwd_kernel<1><<<blocks, 256, 0, st>>>(gy, gx, n, d, h, w, c);
     return mdt::launch_status();
 }
 
