@@ -441,6 +441,32 @@ size_t mdt_eval_patient_workspace_bytes(int n_slots, int n_members);
 int mdt_eval_patient(const double *row_score, const int *row_label, const int *row_slot, int n_rows, int n_slots, const int *seg_offsets,
                      const int *seg_slots, int n_members, int n_seg, double *thr, int *tps, int *fps, int *n_thr, void *ws, size_t ws_bytes,
                      void *stream);
+/* Patient bootstrap.  The units are P = n_patients patients; a row's patient index is in [0, P).  mult [n_boot, P] int32 holds one
+ * resample per row, m[p] in [0, P] (the host draws it: numpy's RandomState([seed, b]).randint(0, P, P), bincount).  A resample's metrics
+ * are by definition those of the materialised resample: every row of patient p repeated m[p] times in place (copies next to each other),
+ * copy j of p a patient of its own, matching not redone.  The kernels never materialise it; every count is an integer sum of weights and
+ * the outputs equal the evaluation of the materialised rows bit for bit (the argument is in csrc/evaluate.cu).  Both entries check the
+ * patient indices and multiplicities on the device and wait for that check (one synchronisation of `stream`): MDT_EINVAL when one is out
+ * of range, and also when n_patients * n_rows >= 2^31 (the bound on every weighted count), on negative sizes or n_recall / n_rates > 128.
+ * n_boot = 0 does nothing.
+ *
+ * mdt_eval_bootstrap_roi: rows as mdt_eval_roi_ap's plus row_patient; one threshold (detections with score > threshold; NaN scores left
+ * out); recall_points ascending.  Per (resample b, segment s), o = b * n_seg + s: q [o, n_recall] as mdt_eval_roi_ap's, counts [o, 2] =
+ * (weighted all_p, weighted nd), froc_tp [o, n_rates] = max{TP(v) : FP(v) <= fp_limits[f]} over the operating points (origin and, per
+ * distinct score v above the threshold, the weighted TP / FP detections with score >= v): the step FROC, no interpolation between points.
+ * The sensitivity is froc_tp / all_p (all_p = det_tp + det_fn rows, the GT lesions); fp_limits [n_rates] = rate * P, fp64. */
+size_t mdt_eval_bootstrap_roi_workspace_bytes(int n_rows, int n_seg, int n_patients);
+int mdt_eval_bootstrap_roi(const double *row_score, const int *row_seg, const int *row_kind, const int *row_patient, int n_rows, int n_seg,
+                           int n_patients, const int *mult, int n_boot, double threshold, const double *recall_points, int n_recall,
+                           const double *fp_limits, int n_rates, double *q, int *counts, int *froc_tp, void *ws, size_t ws_bytes, void *stream);
+/* mdt_eval_bootstrap_patient: rows, slots and segments as mdt_eval_patient's plus row_patient (the rows of one slot share a patient);
+ * n_patients * n_members < 2^31.  Per resample b and segment k, the distinct thresholds with nonzero weight in descending order with the
+ * weighted tps / fps at each, written from b * n_members + seg_offsets[k] on; n_thr [n_boot, n_seg]. */
+size_t mdt_eval_bootstrap_patient_workspace_bytes(int n_slots, int n_members, int n_seg);
+int mdt_eval_bootstrap_patient(const double *row_score, const int *row_label, const int *row_slot, const int *row_patient, int n_rows,
+                               int n_slots, const int *seg_offsets, const int *seg_slots, int n_members, int n_seg, int n_patients,
+                               const int *mult, int n_boot, double *thr, int *tps, int *fps, int *n_thr, void *ws, size_t ws_bytes,
+                               void *stream);
 
 /* ------------------------------------------------------------- data loader (csrc/loader.cu) -----------------------------------------------
  * replaces: the volume scans of BatchGenerator.generate_train_batch and the tiling of PatientBatchIterator.generate_train_batch in

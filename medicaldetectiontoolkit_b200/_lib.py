@@ -128,6 +128,10 @@ SIGNATURES = {
     "mdt_eval_roi_ap": (_I, [_VP, _VP, _VP, _I, _I, _VP, _I, _VP, _I, _VP, _VP, _VP, _SZ, _VP]),
     "mdt_eval_patient_workspace_bytes": (_SZ, [_I, _I]),
     "mdt_eval_patient": (_I, [_VP, _VP, _VP, _I, _I, _VP, _VP, _I, _I, _VP, _VP, _VP, _VP, _VP, _SZ, _VP]),
+    "mdt_eval_bootstrap_roi_workspace_bytes": (_SZ, [_I, _I, _I]),
+    "mdt_eval_bootstrap_roi": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _VP, _I, _D, _VP, _I, _VP, _I, _VP, _VP, _VP, _VP, _SZ, _VP]),
+    "mdt_eval_bootstrap_patient_workspace_bytes": (_SZ, [_I, _I, _I]),
+    "mdt_eval_bootstrap_patient": (_I, [_VP, _VP, _VP, _VP, _I, _I, _VP, _VP, _I, _I, _I, _VP, _I, _VP, _VP, _VP, _VP, _VP, _SZ, _VP]),
     "mdt_unmold_masks": (_I, [_I, _VP, _I, _VP, c_i64p, _I, ctypes.POINTER(_I), _I, ctypes.POINTER(_I), _VP, _VP, _VP]),
     "mdt_loader_fg_index_workspace_bytes": (_SZ, [_I, _I, _I]),
     "mdt_loader_fg_index": (_I, [_VP, _I, _I, _I, _VP, _VP, _I, _VP, _SZ, _VP]),

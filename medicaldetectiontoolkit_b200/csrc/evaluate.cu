@@ -203,6 +203,28 @@ __global__ void ap_gather_kernel(const int *perm, const int *seg_sorted, const d
     if (k == n - 1 || seg_sorted[k + 1] != s) seg_end[s] = k + 1;
 }
 
+// The reverse-max precision envelope read at the recall points, shared by the ROI AP and its bootstrap.  idx[r] is the searchsorted
+// position of recall point r (non-decreasing in r); the interval of a detection at position k is the last r with idx[r] <= k, and the
+// envelope at r, max(pr[idx[r]:nd]), is the suffix maximum over the intervals from r on.  pr >= 0, so its fp64 bit patterns order like
+// the values and an integer atomicMax is exact and order-independent.
+__device__ __forceinline__ void envelope_add(const int *s_idx, unsigned long long *s_pm, int n_r, int k, double pr) {
+    int lo = 0, hi = n_r;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (s_idx[mid] <= k) lo = mid + 1;
+        else hi = mid;
+    }
+    if (lo > 0) atomicMax(&s_pm[lo - 1], (unsigned long long)__double_as_longlong(pr));   // before idx[0]: in no interval
+}
+
+__device__ __forceinline__ void envelope_write(const int *s_idx, const unsigned long long *s_pm, int n_r, int nd, double *out) {
+    unsigned long long run = 0ull;
+    for (int r = n_r - 1; r >= 0; --r) {
+        if (s_pm[r] > run) run = s_pm[r];
+        out[r] = s_idx[r] < nd ? __longlong_as_double((long long)run) : 0.0;   // past the last detection: the try/except leaves 0
+    }
+}
+
 __global__ void __launch_bounds__(kApThreads) ap_kernel(const double *ss, const int *tpc, const int *seg_start, const int *seg_end,
                                                         const int *all_p, const double *thresh, int n_thresh, const double *recall, int n_r,
                                                         double *q, int *counts) {
@@ -239,24 +261,10 @@ __global__ void __launch_bounds__(kApThreads) ap_kernel(const double *ss, const 
         s_idx[r] = lo;
     }
     __syncthreads();
-    for (int k = s_idx[0] + tid; k < nd; k += kApThreads) {
-        int lo = 0, hi = n_r;                          // interval of k: the last r with idx[r] <= k (>= 0 since idx[0] <= k)
-        while (lo < hi) {
-            const int mid = (lo + hi) >> 1;
-            if (s_idx[mid] <= k) lo = mid + 1;
-            else hi = mid;
-        }
-        const double pr = __ddiv_rn((double)tpc[b + k], (double)(k + 1));
-        atomicMax(&s_pm[lo - 1], (unsigned long long)__double_as_longlong(pr));
-    }
+    for (int k = s_idx[0] + tid; k < nd; k += kApThreads) envelope_add(s_idx, s_pm, n_r, k, __ddiv_rn((double)tpc[b + k], (double)(k + 1)));
     __syncthreads();
     if (tid == 0) {
-        double *out = q + ((size_t)seg * n_thresh + ti) * n_r;
-        unsigned long long run = 0ull;
-        for (int r = n_r - 1; r >= 0; --r) {
-            if (s_pm[r] > run) run = s_pm[r];
-            out[r] = s_idx[r] < nd ? __longlong_as_double((long long)run) : 0.0;   // past the last detection: the try/except leaves 0
-        }
+        envelope_write(s_idx, s_pm, n_r, nd, q + ((size_t)seg * n_thresh + ti) * n_r);
         counts[(size_t)seg * (1 + n_thresh) + 1 + ti] = nd;
         if (ti == 0) counts[(size_t)seg * (1 + n_thresh)] = ap;
     }
@@ -345,6 +353,322 @@ size_t ap_cub_bytes(int n, int n_seg) {
     return a > b ? (a > c ? a : c) : (b > c ? b : c);
 }
 
+
+// The workspace of the ROI sort, shared by mdt_eval_roi_ap and mdt_eval_bootstrap_roi: the rows of every segment in (score descending,
+// row order), with per-segment [seg_start, seg_end) and the unweighted all_p.  aux [n] is the caller's: the TP prefix counts of the ROI AP,
+// the patient index of each sorted row in the bootstrap.
+struct RoiSort {
+    double *key_out, *ss;
+    int *iota, *perm_desc, *seg_key, *seg_sorted, *perm, *is_tp, *aux, *all_p, *seg_start, *seg_end;
+    void *tmp;
+    size_t tmp_b;
+};
+
+size_t roi_sort_bytes(int n, int n_seg) {
+    const size_t cub_b = ap_cub_bytes(n, n_seg);
+    if (cub_b == 0) return 0;
+    const size_t ni = al16((size_t)n * sizeof(int)), nd = al16((size_t)n * sizeof(double));
+    return 2 * nd + 7 * ni + 3 * al16((size_t)n_seg * sizeof(int)) + al16(cub_b);
+}
+
+RoiSort roi_sort_carve(void *ws, int n, int n_seg, size_t bytes) {
+    const size_t ni = al16((size_t)n * sizeof(int)), ndb = al16((size_t)n * sizeof(double)), ns = al16((size_t)n_seg * sizeof(int));
+    char *w = reinterpret_cast<char *>(ws);
+    RoiSort r;
+    r.key_out = reinterpret_cast<double *>(w);
+    r.ss = reinterpret_cast<double *>(w + ndb);
+    int *iw = reinterpret_cast<int *>(w + 2 * ndb);
+    const size_t nie = ni / sizeof(int);
+    r.iota = iw;
+    r.perm_desc = iw + nie;
+    r.seg_key = iw + 2 * nie;
+    r.seg_sorted = iw + 3 * nie;
+    r.perm = iw + 4 * nie;
+    r.is_tp = iw + 5 * nie;
+    r.aux = iw + 6 * nie;
+    r.all_p = reinterpret_cast<int *>(w + 2 * ndb + 7 * ni);
+    r.seg_start = reinterpret_cast<int *>(w + 2 * ndb + 7 * ni + ns);
+    r.seg_end = reinterpret_cast<int *>(w + 2 * ndb + 7 * ni + 2 * ns);
+    r.tmp = w + 2 * ndb + 7 * ni + 3 * ns;
+    r.tmp_b = bytes - (2 * ndb + 7 * ni + 3 * ns);
+    return r;
+}
+
+__global__ void ap_gather_patient_kernel(const int *perm, const int *row_patient, int n, int *pat_sorted) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k < n) pat_sorted[k] = row_patient[perm[k]];
+}
+
+// Two stable cub radix sorts (score descending, then segment id); with row_patient, also the patient index of every sorted row into aux
+int roi_sort(const RoiSort &r, const double *row_score, const int *row_seg, const int *row_kind, const int *row_patient, int n_rows,
+             int n_seg, cudaStream_t st) {
+    if (cudaMemsetAsync(r.all_p, 0, 3 * al16((size_t)n_seg * sizeof(int)), st) != cudaSuccess) return launch_status();
+    if (n_rows == 0) return MDT_OK;
+    const int blk = 256, grid = (n_rows + blk - 1) / blk;
+    size_t tmp_b = r.tmp_b;
+    ap_iota_kernel<<<grid, blk, 0, st>>>(r.iota, n_rows);
+    if (cub::DeviceRadixSort::SortPairsDescending(r.tmp, tmp_b, row_score, r.key_out, r.iota, r.perm_desc, n_rows, 0, 64, st) != cudaSuccess)
+        return launch_status();
+    ap_prepare_kernel<<<grid, blk, 0, st>>>(r.perm_desc, row_score, row_seg, row_kind, n_rows, n_seg, r.all_p, r.seg_key);
+    tmp_b = r.tmp_b;
+    if (cub::DeviceRadixSort::SortPairs(r.tmp, tmp_b, r.seg_key, r.seg_sorted, r.perm_desc, r.perm, n_rows, 0, seg_bits(n_seg), st) !=
+        cudaSuccess)
+        return launch_status();
+    ap_gather_kernel<<<grid, blk, 0, st>>>(r.perm, r.seg_sorted, row_score, row_kind, n_rows, n_seg, r.ss, r.is_tp, r.seg_start, r.seg_end);
+    if (row_patient) ap_gather_patient_kernel<<<grid, blk, 0, st>>>(r.perm, row_patient, n_rows, r.aux);
+    return launch_status();
+}
+
+
+// ------------------------------------------------------------------------------------------------------------------------------ bootstrap
+// A resample gives patient p the multiplicity m[p] >= 0; its metrics are by definition those of the materialised resample, where every
+// row of p is repeated m[p] times in place (copies next to each other) and copy j of p is a patient of its own.  The kernels never
+// materialise it: every count is a sum of integer weights, and the points that decide each metric are read off the weighted prefix sums.
+//
+// ROI AP.  In (score descending, row order) the materialised detections are the original ones with row i repeated w_i = m[pat(i)] times
+// in place.  Let W_i / T_i be the weighted detections / TPs up to and including row i.  The m copies of a TP row sit at positions
+// W_i - m .. W_i - 1 with precision (T_i - m + j) / (W_i - m + j), j = 1..m, which rises with j: whenever the suffix max(pr[idx:nd]) sees a
+// copy it also sees the last one, which is the largest, so only the last copy (position W_i - 1, precision T_i / W_i) can carry the
+// envelope.  The copies of an FP row keep the TP count and lower the precision with every copy, so only the first (position W_{i-1},
+// precision T_i / (W_{i-1} + 1)) can; and a searchsorted position never falls strictly inside an FP run, because the recall there equals
+// the recall one position earlier.  The recall point r is first reached at the c*-th TP, c* = the least count with c* / all_p >= R[r]
+// (fp64 division is monotone in the numerator), i.e. at copy c* - T_{i-1} of the TP row with T_{i-1} < c* <= T_i.  So the weighted scan
+// feeds the shared envelope rule exactly the positions and fp64 precisions (integer / integer) that decide numpy's envelope on the
+// materialised rows, and the outputs are bit-identical to it.  Rows with w = 0 add nothing.
+//
+// FROC.  The operating points are (TP(v), FP(v)) at the ends of the runs of equal score (a run never straddles the threshold); a run of
+// zero-weight rows repeats the previous point, which changes no maximum.  TP and FP only grow along the order, so the sensitivity at an FP
+// limit is the TP count of the last run end within the limit: an integer max per rate (warp max, then a shared atomicMax).
+//
+// Patient level.  Per segment the members (slots) are sorted once by score descending; per resample a slot weighs m of its patient.  A run
+// of equal scores is a distinct threshold of the resample when its weight is nonzero, i.e. when the weighted count at its end exceeds the
+// count at the previous run end; its tps / fps are the weighted prefix counts there.
+constexpr int kBootThreads = 256;
+
+// (W, T) packed in one 64-bit sum, W in the high word: both stay below 2^31 (n_patients * n_rows < 2^31 and m <= n_patients)
+__device__ __forceinline__ unsigned long long pack2(int hi, int lo) { return ((unsigned long long)(unsigned)hi << 32) | (unsigned)lo; }
+
+// *bad = 1 when a row's patient index is outside [0, P) or a multiplicity outside [0, P]
+__global__ void boot_check_kernel(const int *row_patient, int n_rows, const int *mult, long long n_mult, int P, int *bad) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    bool b = false;
+    if (i < n_rows) b = row_patient[i] < 0 || row_patient[i] >= P;
+    if (i < n_mult) b = b || mult[i] < 0 || mult[i] > P;
+    if (b) atomicOr(bad, 1);
+}
+
+// npos[seg, p] = rows of type TP / FN of patient p in segment seg (integer atomics: order-independent)
+__global__ void boot_npos_kernel(const int *row_seg, const int *row_kind, const int *row_patient, int n, int n_seg, int P, int *npos) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int s = row_seg[i], t = row_kind[i];
+    if (s >= 0 && s < n_seg && (t == kTp || t == kFn)) atomicAdd(&npos[(size_t)s * P + row_patient[i]], 1);
+}
+
+// one block per (resample, segment): weighted all_p, two passes of a (W, T) block scan over the detections above the threshold
+__global__ void __launch_bounds__(kBootThreads) boot_roi_kernel(const double *ss, const int *is_tp, const int *pat, const int *seg_start,
+                                                                const int *seg_end, const int *npos, int n_seg, int P, const int *mult,
+                                                                double th, const double *recall, int n_r, const double *fp_lim, int n_rates,
+                                                                double *q, int *counts, int *froc_tp) {
+    using Scan = cub::BlockScan<unsigned long long, kBootThreads>;
+    using Reduce = cub::BlockReduce<int, kBootThreads>;
+    __shared__ union {
+        typename Scan::TempStorage scan;
+        typename Reduce::TempStorage reduce;
+    } tmp;
+    __shared__ int s_c[kMaxRecall], s_idx[kMaxRecall], s_froc[kMaxRecall];
+    __shared__ unsigned long long s_pm[kMaxRecall];
+    __shared__ int s_na, s_ap;
+    const int seg = blockIdx.x % n_seg, tid = threadIdx.x;
+    const size_t o = blockIdx.x, rs = blockIdx.x / n_seg;
+    const int *m = mult + rs * P;
+    const int b = seg_start[seg], e = seg_end[seg];
+    int ap = 0;
+    for (int p = tid; p < P; p += kBootThreads) ap += m[p] * npos[(size_t)seg * P + p];
+    ap = Reduce(tmp.reduce).Sum(ap);
+    if (tid == 0) {
+        s_ap = ap;
+        int lo = b, hi = e;              // the rows with score > th: a prefix, scores descend
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (ss[mid] > th) lo = mid + 1;
+            else hi = mid;
+        }
+        s_na = lo;
+    }
+    for (int f = tid; f < n_rates; f += kBootThreads) s_froc[f] = 0;           // the origin (0, 0)
+    __syncthreads();
+    ap = s_ap;
+    const int end = s_na;
+    for (int r = tid; r < n_r; r += kBootThreads) {
+        s_pm[r] = 0ull;
+        s_idx[r] = -1;
+        int lo = 0, hi = ap + 1;         // c*: the least TP count with c* / all_p >= R[r]; all_p + 1: never (and 1 when all_p = 0, no TP)
+        if (ap > 0) {
+            const double R = recall[r], dap = (double)ap;
+            while (lo < hi) {
+                const int mid = (lo + hi) >> 1;
+                if (__ddiv_rn((double)mid, dap) < R) lo = mid + 1;
+                else hi = mid;
+            }
+        }
+        s_c[r] = lo;
+    }
+    __syncthreads();
+    unsigned long long carry = 0ull;
+    for (int c0 = b; c0 < end; c0 += kBootThreads) {      // pass 1: searchsorted positions and FROC
+        const int i = c0 + tid;
+        const bool in = i < end;
+        const int w = in ? m[pat[i]] : 0, tp = in ? is_tp[i] : 0;
+        unsigned long long v, agg;
+        Scan(tmp.scan).InclusiveSum(pack2(w, tp ? w : 0), v, agg);
+        __syncthreads();
+        v += carry;
+        carry += agg;
+        const int W = (int)(v >> 32), T = (int)(v & 0xffffffffull);
+        if (in && tp && w > 0) {
+            const int Tp = T - w, Wp = W - w;
+            int lo = 0, hi = n_r;
+            while (lo < hi) {
+                const int mid = (lo + hi) >> 1;
+                if (s_c[mid] <= Tp) lo = mid + 1;
+                else hi = mid;
+            }
+            for (int r = lo; r < n_r && s_c[r] <= T; ++r) s_idx[r] = Wp + (s_c[r] - Tp) - 1;
+        }
+        const bool run_end = in && (i + 1 == end || ss[i + 1] != ss[i]);
+        for (int f = 0; f < n_rates; ++f) {
+            const int t = __reduce_max_sync(0xffffffffu, run_end && (double)(W - T) <= fp_lim[f] ? T : 0);
+            if ((tid & 31) == 0 && t > 0) atomicMax(&s_froc[f], t);
+        }
+    }
+    const int nd = (int)(carry >> 32);
+    __syncthreads();
+    for (int r = tid; r < n_r; r += kBootThreads)
+        if (s_idx[r] < 0) s_idx[r] = s_c[r] == 0 ? 0 : nd;    // c* = 0: position 0; beyond the TPs above the threshold: nd
+    __syncthreads();
+    carry = 0ull;
+    for (int c0 = b; c0 < end; c0 += kBootThreads) {      // pass 2: the envelope from each row's deciding copy
+        const int i = c0 + tid;
+        const bool in = i < end;
+        const int w = in ? m[pat[i]] : 0, tp = in ? is_tp[i] : 0;
+        unsigned long long v, agg;
+        Scan(tmp.scan).InclusiveSum(pack2(w, tp ? w : 0), v, agg);
+        __syncthreads();
+        v += carry;
+        carry += agg;
+        const int W = (int)(v >> 32), T = (int)(v & 0xffffffffull);
+        if (in && w > 0) {
+            if (tp) envelope_add(s_idx, s_pm, n_r, W - 1, __ddiv_rn((double)T, (double)W));
+            else envelope_add(s_idx, s_pm, n_r, W - w, __ddiv_rn((double)T, (double)(W - w + 1)));
+        }
+    }
+    __syncthreads();
+    if (tid == 0) {
+        envelope_write(s_idx, s_pm, n_r, nd, q + o * n_r);
+        counts[2 * o] = ap;
+        counts[2 * o + 1] = nd;
+    }
+    for (int f = tid; f < n_rates; f += kBootThreads) froc_tp[o * n_rates + f] = s_froc[f];
+}
+
+__global__ void boot_slot_patient_kernel(const int *row_slot, const int *row_patient, int n, int n_slots, int *s_pat) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int s = row_slot[i];
+    if (s >= 0 && s < n_slots) atomicMax(&s_pat[s], row_patient[i]);
+}
+
+// the sort keys of the members: the slot's ordered score key, or 0 (sorts last) with slot -1 for a member that is not a patient
+__global__ void boot_member_keys_kernel(const int *seg_slots, int n_members, int n_slots, const int *s_label, const unsigned long long *s_key,
+                                        unsigned long long *key, int *slot) {
+    const int a = blockIdx.x * blockDim.x + threadIdx.x;
+    if (a >= n_members) return;
+    const int sa = seg_slots[a];
+    const bool ok = sa >= 0 && sa < n_slots && s_label[sa] >= 0;
+    key[a] = ok ? s_key[sa] : 0ull;
+    slot[a] = ok ? sa : -1;
+}
+
+// one block per (resample, segment) over the segment's members in descending score: (tps, fps) block scan, the previous run end's
+// weighted count by an exclusive max scan, the emitted thresholds' ranks by an exclusive sum
+__global__ void __launch_bounds__(kBootThreads) boot_pat_kernel(const unsigned long long *key, const int *slot, const int *s_label,
+                                                                const int *s_pat, const int *seg_off, int n_seg, int n_members, int P,
+                                                                const int *mult, double *thr, int *tps, int *fps, int *n_thr) {
+    using ScanU = cub::BlockScan<unsigned long long, kBootThreads>;
+    using ScanI = cub::BlockScan<int, kBootThreads>;
+    __shared__ union {
+        typename ScanU::TempStorage u;
+        typename ScanI::TempStorage i;
+    } tmp;
+    const int seg = blockIdx.x % n_seg, tid = threadIdx.x;
+    const size_t rs = blockIdx.x / n_seg;
+    const int *m = mult + rs * P;
+    const int b = seg_off[seg], e = seg_off[seg + 1];
+    const size_t out = rs * n_members;
+    unsigned long long carry = 0ull;
+    int last_end = 0, n_out = 0;
+    for (int c0 = b; c0 < e; c0 += kBootThreads) {
+        const int a = c0 + tid;
+        const bool in = a < e;
+        int w = 0, pos = 0;
+        double v = 0.0;
+        if (in) {
+            const int sl = slot[a];
+            if (sl >= 0) {
+                w = m[s_pat[sl]];
+                pos = s_label[sl] == 1;
+            }
+            v = key_value(key[a]);
+        }
+        unsigned long long u, agg;
+        ScanU(tmp.u).InclusiveSum(pack2(pos ? w : 0, pos ? 0 : w), u, agg);
+        __syncthreads();
+        u += carry;
+        carry += agg;
+        const int tp = (int)(u >> 32), fp = (int)(u & 0xffffffffull), W = tp + fp;
+        const bool run_end = in && (a + 1 == e || key_value(key[a + 1]) != v);
+        int prev, agg_end;
+        ScanI(tmp.i).ExclusiveScan(run_end ? W : 0, prev, last_end, cub::Max(), agg_end);
+        __syncthreads();
+        last_end = max(last_end, agg_end);
+        const int emit = run_end && W > prev;
+        int rank, n_emit;
+        ScanI(tmp.i).ExclusiveSum(emit, rank, n_emit);
+        __syncthreads();
+        if (emit) {
+            const size_t k = out + b + n_out + rank;
+            thr[k] = v;
+            tps[k] = tp;
+            fps[k] = fp;
+        }
+        n_out += n_emit;
+    }
+    if (tid == 0) n_thr[rs * n_seg + seg] = n_out;
+}
+
+size_t boot_segsort_bytes(int n_members, int n_seg) {
+    size_t t = 0;
+    if (cub::DeviceSegmentedRadixSort::SortPairsDescending(nullptr, t, (const unsigned long long *)nullptr, (unsigned long long *)nullptr,
+                                                           (const int *)nullptr, (int *)nullptr, n_members, n_seg, (const int *)nullptr,
+                                                           (const int *)nullptr) != cudaSuccess)
+        return 0;
+    return t > 0 ? t : 16;
+}
+
+// the device check of the patient indices and multiplicities; waits for it (one stream synchronisation)
+int boot_check(const int *row_patient, int n_rows, const int *mult, long long n_mult, int P, int *flag, cudaStream_t st) {
+    if (cudaMemsetAsync(flag, 0, sizeof(int), st) != cudaSuccess) return launch_status();
+    const long long n = n_rows > n_mult ? n_rows : n_mult;
+    if (n > 0) boot_check_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(row_patient, n_rows, mult, n_mult, P, flag);
+    int rc = launch_status();
+    if (rc) return rc;
+    int h = 0;
+    if (cudaMemcpyAsync(&h, flag, sizeof(int), cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
+        return launch_status();
+    return h ? MDT_EINVAL : MDT_OK;
+}
+
 }  // namespace
 }  // namespace mdt
 
@@ -393,10 +717,7 @@ int mdt_eval_match(const double *cand_boxes, const double *cand_scores, const in
 
 size_t mdt_eval_roi_ap_workspace_bytes(int n_rows, int n_seg) {
     if (n_rows <= 0 || n_seg <= 0) return 0;
-    const size_t cub_b = mdt::ap_cub_bytes(n_rows, n_seg);
-    if (cub_b == 0) return 0;
-    const size_t ni = mdt::al16((size_t)n_rows * sizeof(int)), nd = mdt::al16((size_t)n_rows * sizeof(double));
-    return 2 * nd + 7 * ni + 3 * mdt::al16((size_t)n_seg * sizeof(int)) + mdt::al16(cub_b);
+    return mdt::roi_sort_bytes(n_rows, n_seg);
 }
 
 int mdt_eval_roi_ap(const double *row_score, const int *row_seg, const int *row_kind, int n_rows, int n_seg, const double *thresholds,
@@ -410,37 +731,14 @@ int mdt_eval_roi_ap(const double *row_score, const int *row_seg, const int *row_
     if (need == 0) return MDT_EDRIVER;
     if (ws_bytes < need) return MDT_EWORKSPACE;
     cudaStream_t st = mdt::as_stream(stream);
-    const size_t ni = mdt::al16((size_t)n * sizeof(int)), ndb = mdt::al16((size_t)n * sizeof(double)), ns = mdt::al16((size_t)n_seg * sizeof(int));
-    char *w = reinterpret_cast<char *>(ws);
-    double *key_out = reinterpret_cast<double *>(w);
-    double *ss = reinterpret_cast<double *>(w + ndb);
-    int *iota = reinterpret_cast<int *>(w + 2 * ndb);
-    int *perm_desc = reinterpret_cast<int *>(w + 2 * ndb + ni);
-    int *seg_key = reinterpret_cast<int *>(w + 2 * ndb + 2 * ni);
-    int *seg_sorted = reinterpret_cast<int *>(w + 2 * ndb + 3 * ni);
-    int *perm = reinterpret_cast<int *>(w + 2 * ndb + 4 * ni);
-    int *is_tp = reinterpret_cast<int *>(w + 2 * ndb + 5 * ni);
-    int *tpc = reinterpret_cast<int *>(w + 2 * ndb + 6 * ni);
-    int *all_p = reinterpret_cast<int *>(w + 2 * ndb + 7 * ni);
-    int *seg_start = reinterpret_cast<int *>(w + 2 * ndb + 7 * ni + ns);
-    int *seg_end = reinterpret_cast<int *>(w + 2 * ndb + 7 * ni + 2 * ns);
-    void *tmp = w + 2 * ndb + 7 * ni + 3 * ns;
-    size_t tmp_b = need - (2 * ndb + 7 * ni + 3 * ns);
-    if (cudaMemsetAsync(all_p, 0, 3 * ns, st) != cudaSuccess) return mdt::launch_status();
-    if (n_rows > 0) {
-        const int blk = 256, grid = (n_rows + blk - 1) / blk;
-        mdt::ap_iota_kernel<<<grid, blk, 0, st>>>(iota, n_rows);
-        if (cub::DeviceRadixSort::SortPairsDescending(tmp, tmp_b, row_score, key_out, iota, perm_desc, n_rows, 0, 64, st) != cudaSuccess)
-            return mdt::launch_status();
-        mdt::ap_prepare_kernel<<<grid, blk, 0, st>>>(perm_desc, row_score, row_seg, row_kind, n_rows, n_seg, all_p, seg_key);
-        if (cub::DeviceRadixSort::SortPairs(tmp, tmp_b, seg_key, seg_sorted, perm_desc, perm, n_rows, 0, mdt::seg_bits(n_seg), st) != cudaSuccess)
-            return mdt::launch_status();
-        mdt::ap_gather_kernel<<<grid, blk, 0, st>>>(perm, seg_sorted, row_score, row_kind, n_rows, n_seg, ss, is_tp, seg_start, seg_end);
-        if (cub::DeviceScan::InclusiveSumByKey(tmp, tmp_b, seg_sorted, is_tp, tpc, n_rows, cub::Equality(), st) != cudaSuccess)
-            return mdt::launch_status();
-    }
-    mdt::ap_kernel<<<n_seg * n_thresh, mdt::kApThreads, 0, st>>>(ss, tpc, seg_start, seg_end, all_p, thresholds, n_thresh, recall_points, n_recall,
-                                                                  q, counts);
+    const mdt::RoiSort rs = mdt::roi_sort_carve(ws, n, n_seg, need);
+    int rc = mdt::roi_sort(rs, row_score, row_seg, row_kind, nullptr, n_rows, n_seg, st);
+    if (rc) return rc;
+    size_t tmp_b = rs.tmp_b;
+    if (n_rows > 0 && cub::DeviceScan::InclusiveSumByKey(rs.tmp, tmp_b, rs.seg_sorted, rs.is_tp, rs.aux, n_rows, cub::Equality(), st) != cudaSuccess)
+        return mdt::launch_status();
+    mdt::ap_kernel<<<n_seg * n_thresh, mdt::kApThreads, 0, st>>>(rs.ss, rs.aux, rs.seg_start, rs.seg_end, rs.all_p, thresholds, n_thresh,
+                                                                  recall_points, n_recall, q, counts);
     return mdt::launch_status();
 }
 
@@ -472,6 +770,103 @@ int mdt_eval_patient(const double *row_score, const int *row_label, const int *r
         if (rc) return rc;
     }
     mdt::pat_curve_kernel<<<n_seg, mdt::kPatThreads, 0, st>>>(s_label, s_key, seg_offsets, seg_slots, n_slots, thr, tps, fps, n_thr, rep);
+    return mdt::launch_status();
+}
+
+size_t mdt_eval_bootstrap_roi_workspace_bytes(int n_rows, int n_seg, int n_patients) {
+    if (n_rows <= 0 || n_seg <= 0 || n_patients <= 0) return 0;
+    const size_t sort_b = mdt::roi_sort_bytes(n_rows, n_seg);
+    if (sort_b == 0) return 0;
+    return sort_b + mdt::al16((size_t)n_seg * n_patients * sizeof(int)) + 16;
+}
+
+int mdt_eval_bootstrap_roi(const double *row_score, const int *row_seg, const int *row_kind, const int *row_patient, int n_rows, int n_seg,
+                           int n_patients, const int *mult, int n_boot, double threshold, const double *recall_points, int n_recall,
+                           const double *fp_limits, int n_rates, double *q, int *counts, int *froc_tp, void *ws, size_t ws_bytes,
+                           void *stream) {
+    if (n_rows < 0 || n_seg <= 0 || n_patients <= 0 || n_boot < 0 || n_recall <= 0 || n_recall > mdt::kMaxRecall || n_rates <= 0 ||
+        n_rates > mdt::kMaxRecall)
+        return MDT_EINVAL;
+    if ((long long)n_patients * n_rows >= (1LL << 31) || (long long)n_boot * n_seg >= (1LL << 31)) return MDT_EINVAL;
+    if (!mult || !recall_points || !fp_limits || !q || !counts || !froc_tp || !ws) return MDT_EINVAL;
+    if (n_rows > 0 && (!row_score || !row_seg || !row_kind || !row_patient)) return MDT_EINVAL;
+    if (n_boot == 0) return MDT_OK;
+    const int n = n_rows > 0 ? n_rows : 1;
+    const size_t need = mdt_eval_bootstrap_roi_workspace_bytes(n, n_seg, n_patients);
+    if (need == 0) return MDT_EDRIVER;
+    if (ws_bytes < need) return MDT_EWORKSPACE;
+    cudaStream_t st = mdt::as_stream(stream);
+    const size_t sort_b = mdt::roi_sort_bytes(n, n_seg), npos_b = mdt::al16((size_t)n_seg * n_patients * sizeof(int));
+    char *w = reinterpret_cast<char *>(ws);
+    int *npos = reinterpret_cast<int *>(w + sort_b);
+    int *flag = reinterpret_cast<int *>(w + sort_b + npos_b);
+    int rc = mdt::boot_check(row_patient, n_rows, mult, (long long)n_boot * n_patients, n_patients, flag, st);
+    if (rc) return rc;
+    const mdt::RoiSort rs = mdt::roi_sort_carve(ws, n, n_seg, sort_b);
+    rc = mdt::roi_sort(rs, row_score, row_seg, row_kind, row_patient, n_rows, n_seg, st);
+    if (rc) return rc;
+    if (cudaMemsetAsync(npos, 0, npos_b, st) != cudaSuccess) return mdt::launch_status();
+    if (n_rows > 0) mdt::boot_npos_kernel<<<(n_rows + 255) / 256, 256, 0, st>>>(row_seg, row_kind, row_patient, n_rows, n_seg, n_patients, npos);
+    mdt::boot_roi_kernel<<<n_boot * n_seg, mdt::kBootThreads, 0, st>>>(rs.ss, rs.is_tp, rs.aux, rs.seg_start, rs.seg_end, npos, n_seg, n_patients,
+                                                                       mult, threshold, recall_points, n_recall, fp_limits, n_rates, q, counts,
+                                                                       froc_tp);
+    return mdt::launch_status();
+}
+
+size_t mdt_eval_bootstrap_patient_workspace_bytes(int n_slots, int n_members, int n_seg) {
+    if (n_slots <= 0 || n_members < 0 || n_seg <= 0) return 0;
+    const int nm = n_members > 0 ? n_members : 1;
+    const size_t sort_b = mdt::boot_segsort_bytes(nm, n_seg);
+    if (sort_b == 0) return 0;
+    return 2 * mdt::al16((size_t)n_slots * sizeof(int)) + mdt::al16((size_t)n_slots * sizeof(unsigned long long)) +
+           2 * mdt::al16((size_t)nm * sizeof(unsigned long long)) + 2 * mdt::al16((size_t)nm * sizeof(int)) + 16 + mdt::al16(sort_b);
+}
+
+int mdt_eval_bootstrap_patient(const double *row_score, const int *row_label, const int *row_slot, const int *row_patient, int n_rows,
+                               int n_slots, const int *seg_offsets, const int *seg_slots, int n_members, int n_seg, int n_patients,
+                               const int *mult, int n_boot, double *thr, int *tps, int *fps, int *n_thr, void *ws, size_t ws_bytes,
+                               void *stream) {
+    if (n_rows < 0 || n_slots <= 0 || n_members < 0 || n_seg <= 0 || n_patients <= 0 || n_boot < 0) return MDT_EINVAL;
+    if ((long long)n_patients * n_rows >= (1LL << 31) || (long long)n_patients * n_members >= (1LL << 31) ||
+        (long long)n_boot * n_seg >= (1LL << 31))
+        return MDT_EINVAL;
+    if (!seg_offsets || !mult || !n_thr || !ws || (n_rows > 0 && (!row_score || !row_label || !row_slot || !row_patient))) return MDT_EINVAL;
+    if (n_members > 0 && (!seg_slots || !thr || !tps || !fps)) return MDT_EINVAL;
+    if (n_boot == 0) return MDT_OK;
+    const size_t need = mdt_eval_bootstrap_patient_workspace_bytes(n_slots, n_members, n_seg);
+    if (need == 0) return MDT_EDRIVER;
+    if (ws_bytes < need) return MDT_EWORKSPACE;
+    cudaStream_t st = mdt::as_stream(stream);
+    const int nm = n_members > 0 ? n_members : 1;
+    const size_t si = mdt::al16((size_t)n_slots * sizeof(int)), sk = mdt::al16((size_t)n_slots * sizeof(unsigned long long));
+    const size_t mk = mdt::al16((size_t)nm * sizeof(unsigned long long)), mi = mdt::al16((size_t)nm * sizeof(int));
+    char *w = reinterpret_cast<char *>(ws);
+    int *s_label = reinterpret_cast<int *>(w);
+    int *s_pat = reinterpret_cast<int *>(w + si);
+    unsigned long long *s_key = reinterpret_cast<unsigned long long *>(w + 2 * si);
+    unsigned long long *key = reinterpret_cast<unsigned long long *>(w + 2 * si + sk);
+    unsigned long long *key_sorted = reinterpret_cast<unsigned long long *>(w + 2 * si + sk + mk);
+    int *slot = reinterpret_cast<int *>(w + 2 * si + sk + 2 * mk);
+    int *slot_sorted = reinterpret_cast<int *>(w + 2 * si + sk + 2 * mk + mi);
+    int *flag = reinterpret_cast<int *>(w + 2 * si + sk + 2 * mk + 2 * mi);
+    void *tmp = w + 2 * si + sk + 2 * mk + 2 * mi + 16;
+    size_t tmp_b = need - (2 * si + sk + 2 * mk + 2 * mi + 16);
+    int rc = mdt::boot_check(row_patient, n_rows, mult, (long long)n_boot * n_patients, n_patients, flag, st);
+    if (rc) return rc;
+    if (cudaMemsetAsync(s_label, 0xff, 2 * si, st) != cudaSuccess || cudaMemsetAsync(s_key, 0, sk, st) != cudaSuccess)
+        return mdt::launch_status();
+    if (n_rows > 0) {
+        mdt::pat_reduce_kernel<<<(n_rows + 255) / 256, 256, 0, st>>>(row_score, row_label, row_slot, n_rows, n_slots, s_label, s_key);
+        mdt::boot_slot_patient_kernel<<<(n_rows + 255) / 256, 256, 0, st>>>(row_slot, row_patient, n_rows, n_slots, s_pat);
+    }
+    if (n_members > 0) {
+        mdt::boot_member_keys_kernel<<<(n_members + 255) / 256, 256, 0, st>>>(seg_slots, n_members, n_slots, s_label, s_key, key, slot);
+        if (cub::DeviceSegmentedRadixSort::SortPairsDescending(tmp, tmp_b, key, key_sorted, slot, slot_sorted, n_members, n_seg, seg_offsets,
+                                                               seg_offsets + 1, 0, 64, st) != cudaSuccess)
+            return mdt::launch_status();
+    }
+    mdt::boot_pat_kernel<<<n_boot * n_seg, mdt::kBootThreads, 0, st>>>(key_sorted, slot_sorted, s_label, s_pat, seg_offsets, n_seg, n_members,
+                                                                       n_patients, mult, thr, tps, fps, n_thr);
     return mdt::launch_status();
 }
 

@@ -20,6 +20,9 @@ reference returns.
 Scores and coordinates are promoted to fp64.  Ground-truth coordinates often arrive as integer arrays; the reference computes their
 volumes in int64 and mixes them with fp64, and promoting them to fp64 first gives the same values as long as coordinates and volumes stay
 below 2^53.  For ROI-level ties in score, rows keep their row order (the reference's pandas quicksort leaves it undefined).
+
+Beyond the reference: Evaluator.bootstrap / score_bootstrap give patient-bootstrap confidence intervals and the (step) FROC / CPM of the
+stored rows, each resample evaluated on the device from weighted counts (see Evaluator.bootstrap for the definitions).
 """
 import os
 
@@ -31,6 +34,8 @@ from . import _lib as L
 TYPES = ('det_tp', 'det_fp', 'det_fn', 'patient_tn')      # type codes 0..3 of csrc/evaluate.cu
 RECALL_POINTS = np.linspace(.0, 1, 101, endpoint=True)      # compute_roi_ap's R
 SCAN_THRESHOLDS = list(np.arange(0.9, 1, 0.01))            # return_metrics' conf_threshs
+FROC_RATES = (0.125, 0.25, 0.5, 1, 2, 4, 8)                # false positives per scan of the FROC; their mean sensitivity is the CPM
+BOOTSTRAP_CHUNK_BYTES = 64 << 20                           # bound on the device outputs of one bootstrap call (resamples per call follow)
 _TYPES_ARR = np.array(TYPES, dtype=object)
 
 
@@ -149,6 +154,25 @@ def match_rows(flat, n_classes, ious):
     h = out.fetch()
     n = int(h['n'][0])
     return h['score'][:n].copy(), h['meta'].reshape(-1, 4)[:n].copy()
+
+
+def draw_multiplicities(n_pat, n_resamples, seed):
+    """[n_resamples, n_pat] int32: row b is np.bincount of RandomState([seed, b]).randint(0, n_pat, n_pat), the patient multiplicities of
+    bootstrap resample b (independent of n_resamples)"""
+    mult = np.empty((n_resamples, n_pat), dtype=np.int32)
+    for b in range(n_resamples):
+        mult[b] = np.bincount(np.random.RandomState([seed, b]).randint(0, n_pat, size=n_pat), minlength=n_pat)
+    return mult
+
+
+def bootstrap_interval(values, alpha):
+    """(lo, hi, n_valid): np.percentile(valid, [100 alpha / 2, 100 (1 - alpha / 2)]) over the non-NaN values (NaN, NaN when none)"""
+    v = np.asarray(values, dtype=np.float64).reshape(-1)
+    valid = v[~np.isnan(v)]
+    if valid.size == 0:
+        return np.nan, np.nan, 0
+    lo, hi = np.percentile(valid, [100 * alpha / 2, 100 * (1 - alpha / 2)])
+    return float(lo), float(hi), int(valid.size)
 
 
 def _type_codes(det_type):
@@ -339,6 +363,127 @@ class Evaluator():
                                       .format(s['auc'], s['mean_auc'], s['ap'], s['mean_ap'], s['name'], cf.exp_dir.split('/')[-1]))
                     handle2.write('\n')
 
+    # ------------------------------------------------------------------------------------------------------- bootstrap and FROC
+    def bootstrap(self, n_resamples=1000, seed=0, alpha=0.05, fps_per_scan=FROC_RATES):
+        """Patient-bootstrap confidence intervals of the stored rows' metrics, with FROC and CPM.
+
+        The units are the distinct pids of the rows (np.unique order; several folds' rows are pooled), P of them.  Resample b draws
+        RandomState([seed, b]).randint(0, P, P), so it does not depend on n_resamples; patient p then weighs m[p] = its draw count.  A
+        resample's metrics are those of the materialised resample: every row of p repeated m[p] times in place, copy j of p a patient of
+        its own, the matching not redone.  The kernels (mdt_eval_bootstrap_roi / _patient) compute them from integer weighted counts,
+        bit-identical to the materialised evaluation, and the host applies return_metrics' expressions to their outputs:
+          - ROI AP per class: the mean over the match-IoU segments with all_p > 0 of the 101-point interpolated precision at
+            cf.min_det_thresh (cf.per_patient_ap is not used); average_foreground_roi is the mean over the classes of each resample;
+          - patient AUC / AP per class: return_metrics' curve expressions on the weighted distinct-threshold counts;
+          - FROC per class and match IoU: sens(r) = max{TP(v) : FP(v) <= r * P} / G over the operating points (the origin and, per
+            distinct score v above cf.min_det_thresh, the TP / FP detections with score >= v; NaN scores left out), G the det_tp + det_fn
+            rows, NaN when G = 0.  This is the step FROC: LUNA16's script interpolates linearly between operating points, this one
+            does not.  The CPM is the mean of sens over fps_per_scan.
+        The interval of each metric is np.percentile(valid, [100 alpha / 2, 100 (1 - alpha / 2)]) over the resamples where it is not
+        NaN, n_valid their number.  The point estimate is the metric of the rows themselves (every m = 1).
+
+        Returns a list of dicts named like return_metrics' entries ('fold_{} rois cl_{}', 'fold_{} patient cl_{}',
+        'average_foreground_roi'): 'ap' (and 'auc' at the patient level) and, per match IoU of a 'rois' entry, 'froc'[iou] = {'sens':
+        one stat per rate, 'cpm': stat}, each stat {'value': point estimate, 'ci': (lo, hi), 'n_valid': n}.  The per-resample values are
+        kept in self.bootstrap_values (same names, numpy arrays).  n_resamples = 0 gives the point estimates alone."""
+        c, cf = self._cols, self.cf
+        if c is None or c['pred_score'].size == 0:
+            raise ValueError("bootstrap: no rows are stored (run evaluate_predictions or set test_df first)")
+        if isinstance(n_resamples, bool) or not isinstance(n_resamples, (int, np.integer)) or n_resamples < 0:
+            raise ValueError("bootstrap: n_resamples must be an integer >= 0, got %r" % (n_resamples,))
+        if not 0 < alpha < 1:
+            raise ValueError("bootstrap: alpha must lie in (0, 1), got %r" % (alpha,))
+        rates = np.asarray(fps_per_scan, dtype=np.float64).reshape(-1)
+        if rates.size == 0 or not np.all(np.isfinite(rates) & (rates > 0)):
+            raise ValueError("bootstrap: fps_per_scan must be positive finite rates, got %r" % (fps_per_scan,))
+        n_resamples = int(n_resamples)
+        classes = list(cf.class_dict.keys())
+        levels = list(cf.report_score_level)
+        roi, pat, pat_idx, n_pat = _bootstrap_jobs(c, classes, levels)
+        mult = np.concatenate([np.ones((1, n_pat), dtype=np.int32), draw_multiplicities(n_pat, n_resamples, seed)])
+        roi_ious = {key: _unique_in_order(c['match_iou'][idx])[0] for key, idx in zip(roi.jobs, roi.rows)}
+        n_members = sum(m.size for m in pat.members)
+        per_resample = roi.n_seg * (8 * RECALL_POINTS.size + 4 * (2 + rates.size)) + 16 * n_members + 4 * len(pat.members)
+        chunk = max(1, BOOTSTRAP_CHUNK_BYTES // max(per_resample, 1))
+
+        names = []
+        vals = {}
+        for cl in classes:
+            for level in levels:
+                name = 'fold_{} {} cl_{}'.format(cf.fold, level, cl)
+                names.append((name, level, cl))
+                if level == 'rois':
+                    vals[name] = {'ap': [], 'froc': {float(i): {'sens': [], 'cpm': []} for i in roi_ious[('all', cl)]}}
+                else:
+                    vals[name] = {'auc': [], 'ap': []}
+        vals['average_foreground_roi'] = {'ap': []}
+        for s0 in range(0, 1 + n_resamples, chunk):
+            res = _run_bootstrap_kernels(roi, pat, pat_idx, n_pat, mult[s0:s0 + chunk], cf.min_det_thresh, rates * n_pat)
+            for b in range(min(chunk, 1 + n_resamples - s0)):
+                roi_aps = []
+                for name, level, cl in names:
+                    v = vals[name]
+                    if level == 'rois':
+                        q, counts = res['q'][b][:, None, :], res['counts'][b]
+                        ap = roi.ap({'q': q, 'counts': counts}, ('all', cl), 0)
+                        v['ap'].append(ap)
+                        roi_aps.append(ap)
+                        base, n = roi.jobs[('all', cl)]
+                        for s, iou in zip(range(base, base + n), v['froc']):
+                            g = counts[s, 0]
+                            sens = res['froc'][b][s] / np.float64(g) if g > 0 else np.full(rates.size, np.nan)
+                            v['froc'][iou]['sens'].append(sens)
+                            v['froc'][iou]['cpm'].append(np.mean(sens))
+                    else:
+                        auc, _, ap, _ = pat.scores({k: res[k][b] for k in ('thr', 'tps', 'fps', 'n_thr')}, ('all', cl))
+                        v['auc'].append(auc)
+                        v['ap'].append(ap)
+                vals['average_foreground_roi']['ap'].append(np.mean(roi_aps))
+
+        def stat(x):
+            x = np.asarray(x, dtype=np.float64)
+            lo, hi, n_valid = bootstrap_interval(x[1:], alpha)
+            return {'value': x[0], 'ci': (lo, hi), 'n_valid': n_valid}
+
+        stats, self.bootstrap_values = [], {}
+        for name, v in list(vals.items()):
+            entry, raw = {'name': name}, {}
+            for k in ('auc', 'ap'):
+                if k in v:
+                    entry[k], raw[k] = stat(v[k]), np.asarray(v[k], dtype=np.float64)[1:]
+            if 'froc' in v:
+                entry['fps_per_scan'] = tuple(rates.tolist())
+                entry['froc'], raw['froc'] = {}, {}
+                for iou, f in v['froc'].items():
+                    sens = np.asarray(f['sens'], dtype=np.float64).reshape(-1, rates.size)
+                    entry['froc'][iou] = {'sens': [stat(sens[:, k]) for k in range(rates.size)], 'cpm': stat(f['cpm'])}
+                    raw['froc'][iou] = {'sens': sens[1:], 'cpm': np.asarray(f['cpm'], dtype=np.float64)[1:]}
+            stats.append(entry)
+            self.bootstrap_values[name] = raw
+        return stats
+
+    def score_bootstrap(self, n_resamples=1000, seed=0, alpha=0.05, fps_per_scan=FROC_RATES):
+        """bootstrap() of the stored rows, appended as text to <exp_dir>/results_bootstrap.txt, one line per metric:
+        '<metric> <point> [<lo>, <hi>] (n <n_valid>) <name>[ iou <match iou>]'.  Returns the stats."""
+        stats = self.bootstrap(n_resamples, seed, alpha, fps_per_scan)
+        n_pat = np.unique(self._cols['pid']).size
+
+        def line(metric, s, name):
+            return '{} {:0.4f} [{:0.4f}, {:0.4f}] (n {}) {}\n'.format(metric, s['value'], s['ci'][0], s['ci'][1], s['n_valid'], name)
+        with open(os.path.join(self.cf.exp_dir, 'results_bootstrap.txt'), 'a') as handle:
+            handle.write('\n****************************\n')
+            handle.write('\nbootstrap of fold {}: {} patients, {} resamples, seed {}, {:g}% intervals\n\n'
+                         .format(self.cf.fold, n_pat, n_resamples, seed, 100 * (1 - alpha)))
+            for s in stats:
+                for k in ('auc', 'ap'):
+                    if k in s:
+                        handle.write(line(k.upper(), s[k], s['name']))
+                for iou, f in s.get('froc', {}).items():
+                    for r, st in zip(s['fps_per_scan'], f['sens']):
+                        handle.write(line('FROC@{:g}'.format(r), st, '{} iou {:g}'.format(s['name'], iou)))
+                    handle.write(line('CPM', f['cpm'], '{} iou {:g}'.format(s['name'], iou)))
+        return stats
+
 
 # ---------------------------------------------------------------------------------------------------------------- metric plumbing
 class _RoiJobs:
@@ -480,4 +625,73 @@ def _run_metric_kernels(roi, pat, thresholds):
     if 'counts' in res:
         res['q'] = res['q'].reshape(roi.n_seg, n_thr, RECALL_POINTS.size)
         res['counts'] = res['counts'].reshape(roi.n_seg, 1 + n_thr)
+    return res
+
+
+def _bootstrap_jobs(c, classes, levels):
+    """(roi, pat, patient index per row, P): one ROI job per class (segments = match IoUs) and one patient job per class, folds pooled"""
+    _, pat_idx = np.unique(c['pid'], return_inverse=True)
+    pat_idx = pat_idx.reshape(-1)
+    codes = _type_codes(c['det_type'])
+    roi, pat = _RoiJobs(c, codes, False), _PatientJobs(c)
+    for cl in classes:
+        cmask = c['pred_class'] == cl
+        if 'rois' in levels:
+            roi.add(('all', cl), cmask & (codes != 3))
+        if 'patient' in levels:
+            pat.add_class(cl, cmask, ())
+    return roi, pat, pat_idx, int(pat_idx.max()) + 1
+
+
+def _run_bootstrap_kernels(roi, pat, pat_idx, n_pat, mult, threshold, fp_limits):
+    """mdt_eval_bootstrap_roi and mdt_eval_bootstrap_patient for the resamples mult [n_boot, n_pat]; one device buffer, one copy back"""
+    c = roi.c
+    dev = _device()
+    lib = L.load()
+    stream = L.stream_ptr()
+    n_boot, n_r, n_rates = mult.shape[0], RECALL_POINTS.size, fp_limits.size
+    n_members = sum(m.size for m in pat.members)
+    specs = []
+    if roi.n_seg:
+        specs += [('q', np.float64, n_boot * roi.n_seg * n_r), ('counts', np.int32, n_boot * roi.n_seg * 2),
+                  ('froc', np.int32, n_boot * roi.n_seg * n_rates)]
+    if pat.members:
+        specs += [('thr', np.float64, n_boot * n_members), ('tps', np.int32, n_boot * n_members), ('fps', np.int32, n_boot * n_members),
+                  ('n_thr', np.int32, n_boot * len(pat.members))]
+    if not specs:
+        return {}
+    out = _Outputs(dev, specs)
+    m = _dev(mult, dev, np.int32)
+    keep = [m]
+    if roi.n_seg:
+        idx = np.concatenate(roi.rows)
+        n = int(idx.size)
+        d = [_dev(c['pred_score'][idx], dev, np.float64), _dev(np.concatenate(roi.segs), dev, np.int32), _dev(roi.codes[idx], dev, np.int32),
+             _dev(pat_idx[idx], dev, np.int32), _dev(RECALL_POINTS, dev, np.float64), _dev(fp_limits, dev, np.float64)]
+        ws = _workspace(lib.mdt_eval_bootstrap_roi_workspace_bytes(max(n, 1), roi.n_seg, n_pat), dev)
+        keep += d + [ws]
+        L.check(lib.mdt_eval_bootstrap_roi(L.ptr(d[0]), L.ptr(d[1]), L.ptr(d[2]), L.ptr(d[3]), n, roi.n_seg, n_pat, L.ptr(m), n_boot,
+                                           float(threshold), L.ptr(d[4]), n_r, L.ptr(d[5]), n_rates, out.ptr('q'), out.ptr('counts'),
+                                           out.ptr('froc'), L.ptr(ws), ws.numel(), stream))
+    if pat.members:
+        n = int(c['pred_score'].size)
+        seg_off = np.zeros(len(pat.members) + 1, dtype=np.int32)
+        seg_off[1:] = np.cumsum([s.size for s in pat.members])
+        d = [_dev(c['pred_score'], dev, np.float64), _dev(c['class_label'], dev, np.int32), _dev(pat.row_slot, dev, np.int32),
+             _dev(pat_idx, dev, np.int32), _dev(seg_off, dev, np.int32),
+             _dev(np.concatenate(pat.members) if n_members else np.zeros(1), dev, np.int32)]
+        ws = _workspace(lib.mdt_eval_bootstrap_patient_workspace_bytes(max(pat.n_slots, 1), n_members, len(pat.members)), dev)
+        keep += d + [ws]
+        L.check(lib.mdt_eval_bootstrap_patient(L.ptr(d[0]), L.ptr(d[1]), L.ptr(d[2]), L.ptr(d[3]), n, max(pat.n_slots, 1), L.ptr(d[4]),
+                                               L.ptr(d[5]), n_members, len(pat.members), n_pat, L.ptr(m), n_boot, out.ptr('thr'),
+                                               out.ptr('tps'), out.ptr('fps'), out.ptr('n_thr'), L.ptr(ws), ws.numel(), stream))
+    res = out.fetch()
+    if roi.n_seg:
+        res['q'] = res['q'].reshape(n_boot, roi.n_seg, n_r)
+        res['counts'] = res['counts'].reshape(n_boot, roi.n_seg, 2)
+        res['froc'] = res['froc'].reshape(n_boot, roi.n_seg, n_rates)
+    if pat.members:
+        for k in ('thr', 'tps', 'fps'):
+            res[k] = res[k][:n_boot * n_members].reshape(n_boot, n_members) if n_members else np.zeros((n_boot, 0), res[k].dtype)
+        res['n_thr'] = res['n_thr'].reshape(n_boot, len(pat.members))
     return res
