@@ -42,15 +42,15 @@ bool make_geo(int n, long long s, int c, int per_sample, Geo &g) {
 size_t partial_bytes(const Geo &g) { return (size_t)g.B * g.chunks * g.C * sizeof(double2); }
 size_t group_bytes(const Geo &g) { return (size_t)g.B * g.C * sizeof(double2); }
 
-// act: 0 none, 1 ReLU, 2 leaky ReLU (slope)
+// act: 0 none, 1 ReLU, 2 leaky ReLU (slope); a NaN passes through, as in torch
 __device__ __forceinline__ float act_fwd(float v, int act, float slope) {
-    if (act == 1) return v > 0.f ? v : 0.f;
+    if (act == 1) return v <= 0.f ? 0.f : v;
     if (act == 2) return v > 0.f ? v : v * slope;
     return v;
 }
-// derivative from the saved OUTPUT (torch's rule for in-place activations): y > 0 -> 1, else 0 / slope
+// derivative from the saved OUTPUT (torch's rule for in-place activations): ReLU y <= 0 -> 0 else 1 (NaN too), leaky ReLU y > 0 -> 1 else slope
 __device__ __forceinline__ float act_grad(float y, int act, float slope) {
-    if (act == 1) return y > 0.f ? 1.f : 0.f;
+    if (act == 1) return y <= 0.f ? 0.f : 1.f;
     if (act == 2) return y > 0.f ? 1.f : slope;
     return 1.f;
 }
@@ -147,7 +147,7 @@ __global__ void stats_finalize_kernel(const double2 *__restrict__ part, Geo g, f
     if (lane != 0) return;
     const double M = (double)g.R, mu = t.x / M;
     double var = t.y / M - mu * mu;
-    var = var > 0.0 ? var : 0.0;
+    var = var < 0.0 ? 0.0 : var;   // rounding can take E[x^2] - mean^2 below 0; a NaN (a NaN or Inf in the group) stays NaN, as in torch
     mean[grp] = (float)mu;
     rstd[grp] = (float)(1.0 / sqrt(var + (double)eps));
     if (running_mean != nullptr) {   // batch norm (B = 1): grp == c
@@ -283,7 +283,7 @@ __global__ void stats_from_sums_kernel(const double2 *__restrict__ rows, int N, 
     }
     const double M = (double)N * (double)s, mu = sa / M;
     double var = sb / M - mu * mu;
-    var = var > 0.0 ? var : 0.0;
+    var = var < 0.0 ? 0.0 : var;   // rounding can take E[x^2] - mean^2 below 0; a NaN (a NaN or Inf in the group) stays NaN, as in torch
     mean[c] = (float)mu;
     rstd[c] = (float)(1.0 / sqrt(var + (double)eps));
     if (running_mean != nullptr) {
