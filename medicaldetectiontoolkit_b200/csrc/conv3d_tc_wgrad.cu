@@ -201,8 +201,17 @@ conv_tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_const
     }
 }
 
-// dw[co, ci, tap] = sum over splits (and over the hi / lo lane halves in mtrick mode) of the partial accumulators
-__global__ void __launch_bounds__(256) wgrad_reduce_kernel(TcWgradParams p, float *__restrict__ dw) {
+// dw[co, ci, tap] = sum over splits (and over the hi / lo lane halves in mtrick mode) of the partial accumulators.
+// One thread per output adds its partials in a fixed order: split by split, and inside a split (K = 2: ksplit) the rows of warpgroup 0, then
+// those of warpgroup 1, each (P = 2: mtrick with two planes) the hi row, then the lo row.  A thread has only a few thousand partials to add
+// and there are only 10^4 - 10^5 outputs, so the time is load latency: the partials of kWgReduceLoads / (K * P) splits are loaded before the
+// first of them is added, which keeps that many loads in flight without changing the order of the additions.
+constexpr int kWgReduceThreads = 64;   // small blocks spread the few outputs of the narrow layers over every SM
+constexpr int kWgReduceLoads = 32;
+
+template <int K, int P>
+__global__ void __launch_bounds__(kWgReduceThreads) wgrad_reduce_kernel(TcWgradParams p, float *__restrict__ dw) {
+    constexpr int R = K * P, U = kWgReduceLoads / R;   // rows per split, splits per batch of loads
     const int ncols = p.KW * p.chunkx;
     const long long total = (long long)p.cout * p.ncb_total * ncols;     // (co, column block, col)
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -214,13 +223,35 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(TcWgradParams p, floa
         const int kw = col / p.chunkx, ci = xc * p.chunkx + col % p.chunkx;
         if (ci >= p.cin) continue;
         const int mt = p.mtrick ? 0 : co / 128, m = p.mtrick ? co : co % 128;
+        const float *slot0 = p.partial + ((size_t)cb * p.mtiles + mt) * (size_t)(128 * p.slot_cols) + col;   // split 0
+        const size_t split_stride = (size_t)p.groups * p.mtiles * 128 * p.slot_cols;
+        size_t row[R];
+#pragma unroll
+        for (int j = 0; j < R; ++j) row[j] = (size_t)(m + 64 * (j / P) + (j % P) * p.co_p) * p.slot_cols;
         float acc = 0.f;
-        for (int sp = 0; sp < p.splits; ++sp) {
-            const float *slot = p.partial + (((size_t)sp * p.groups + cb) * p.mtiles + mt) * (size_t)(128 * p.slot_cols) + col;
-            for (int k = 0; k < (p.ksplit ? 2 : 1); ++k) {
-                acc += slot[(size_t)(m + 64 * k) * p.slot_cols];
-                if (p.mtrick && p.planes > 1) acc += slot[(size_t)(m + 64 * k + p.co_p) * p.slot_cols];
-            }
+        int sp0 = 0;
+        for (; sp0 + U <= p.splits; sp0 += U) {   // whole batches: ptxas issues (almost) all of a batch's loads before its first add
+            float v[U][R];
+#pragma unroll
+            for (int u = 0; u < U; ++u)
+#pragma unroll
+                for (int j = 0; j < R; ++j) v[u][j] = __ldg(slot0 + (size_t)(sp0 + u) * split_stride + row[j]);
+#pragma unroll
+            for (int u = 0; u < U; ++u)
+#pragma unroll
+                for (int j = 0; j < R; ++j) acc += v[u][j];
+        }
+        if (sp0 < p.splits) {                      // the last, partial batch
+            float v[U][R];
+#pragma unroll
+            for (int u = 0; u < U; ++u)
+#pragma unroll
+                for (int j = 0; j < R; ++j) v[u][j] = sp0 + u < p.splits ? __ldg(slot0 + (size_t)(sp0 + u) * split_stride + row[j]) : 0.f;
+#pragma unroll
+            for (int u = 0; u < U; ++u)
+                if (sp0 + u < p.splits)
+#pragma unroll
+                    for (int j = 0; j < R; ++j) acc += v[u][j];
         }
         dw[((size_t)co * p.cin + ci) * p.T + (kd * p.KH + kh) * p.KW + kw] = acc;
     }
@@ -415,7 +446,12 @@ static int conv_tc_wgrad_impl(const ConvGeom &g, const float *x, const float *dy
     if ((rc = launch_wgrad_plan(g, w, planes, grid, smem, st, tmY, tmX, p))) return rc;
     {
         const long long total = (long long)g.cout * w.ncb_total * g.kw * w.chunkx;
-        wgrad_reduce_kernel<<<(unsigned)ceil_div<long long>(total, 256), 256, 0, st>>>(p, dw);
+        const unsigned blocks = (unsigned)ceil_div<long long>(total, kWgReduceThreads);
+        const bool two_rows = p.mtrick && p.planes > 1;   // hi and lo row of each warpgroup's lines
+        if (p.ksplit && two_rows) wgrad_reduce_kernel<2, 2><<<blocks, kWgReduceThreads, 0, st>>>(p, dw);
+        else if (p.ksplit) wgrad_reduce_kernel<2, 1><<<blocks, kWgReduceThreads, 0, st>>>(p, dw);
+        else if (two_rows) wgrad_reduce_kernel<1, 2><<<blocks, kWgReduceThreads, 0, st>>>(p, dw);
+        else wgrad_reduce_kernel<1, 1><<<blocks, kWgReduceThreads, 0, st>>>(p, dw);
         if ((rc = launch_status())) return rc;
     }
     if (db && !dy_presplit) return conv_bias_grad(g, dy, db, reinterpret_cast<uint8_t *>(p.partial) + wg_align(partial_bytes), st);
