@@ -583,6 +583,44 @@ int mdt_petct_normalize(const short *ct, const float *pet, long long n, float *o
 #define MDT_TOY_HOLE_CLEARS_SEG 2
 int mdt_toy_images(const uint32_t *keys, int n, int margin, int radius0, int radius1, int flags, double *img, int *params, void *stream);
 
+/* ------------------------------------------------------------- plot rendering (csrc/render.cu) ---------------------------------------------
+ * replaces: the matplotlib drawing behind plotting.py (imshow, plot, hist, text, savefig's rasteriser); the host (plotting.py) builds the
+ * scene and maps data to integer pixels, these draw it into canvas, a device uint8 [height, width, 3] the caller fills (white) first.
+ *
+ * mdt_render_panel: one image source and where it goes.  src: device pointer to element (0, 0) of an [h, w] view with element strides
+ * stride_y, stride_x; dtype MDT_DTYPE_U8, MDT_DTYPE_F16 or MDT_DTYPE_F32.  Source (r, c) fills [y0 + r s, y0 + (r + 1) s) x
+ * [x0 + c s, x0 + (c + 1) s) of the canvas (s = scale >= 1), clipped to it; panels must not overlap.  A descriptor with another dtype or
+ * mode, h, w or scale < 1 draws nothing.
+ * mdt_render_panel_range: range [n, 2] fp32 (device) = (lo, hi) over the finite values of each panel's source, lo = hi = 0 when it has none.
+ * mdt_render_panels: MDT_RENDER_GREY writes g = min(255, (int)fl(fl(x - lo) / fl(hi - lo)) * 256) (each operation rounded to fp32) as
+ * (g, g, g), or 0 when hi <= lo, from range [n, 2]; MDT_RENDER_CLASS writes palette[clamp((int)x, 0, n_palette - 1)] (device uint8
+ * [n_palette, 3], n_palette >= 1).  Non-finite values keep the canvas.  n <= 65535, else MDT_EUNSUPPORTED.  panels: device array.
+ * mdt_render_prim: kind MDT_PRIM_SEGMENT: (x0, y0) -> (x1, y1), both ends drawn; x-major (|dx| >= |dy|) pixels are
+ * (x, y0 + sgn(dy) floor((2 |dy| t + |dx|) / (2 |dx|))) at step t = |x - x0| (y-major symmetric); with dash_period > 0 only the steps with
+ * (dash_offset + t) mod dash_period < dash_on (dash_on >= 1, dash_offset >= 0).  MDT_PRIM_RECT: [x0, x1) x [y0, y1) blended as
+ * (alpha c + (256 - alpha) dst + 128) >> 8 per channel, 0 <= alpha <= 256.  MDT_PRIM_GLYPH: character code (33 .. 126) of the library's
+ * 6 x 8 bitmap font with its top-left at (x0, y0), each font pixel a scale x scale block.  rgb = 0xRRGGBB.  A primitive with a coordinate
+ * beyond +-2^24 or an argument outside these ranges draws nothing.
+ * mdt_render_prims: draws prims [n_prims] (device) strictly in list order, the last to cover a pixel wins (alpha rectangles blend over
+ * what is there), clipped to the canvas.  ceil(height / 16) <= 65535, else MDT_EUNSUPPORTED.  No atomics: deterministic.  No workspace. */
+#define MDT_RENDER_GREY 0
+#define MDT_RENDER_CLASS 1
+#define MDT_PRIM_SEGMENT 0
+#define MDT_PRIM_RECT 1
+#define MDT_PRIM_GLYPH 2
+typedef struct mdt_render_panel {
+    const void *src;
+    long long stride_y, stride_x;
+    int dtype, h, w, y0, x0, scale, mode, pad;
+} mdt_render_panel;
+typedef struct mdt_render_prim {
+    int kind, x0, y0, x1, y1, rgb, alpha, code, scale, dash_on, dash_period, dash_offset;
+} mdt_render_prim;
+int mdt_render_panel_range(const mdt_render_panel *panels, int n_panels, float *range, void *stream);
+int mdt_render_panels(const mdt_render_panel *panels, int n_panels, const float *range, const unsigned char *palette, int n_palette,
+                      unsigned char *canvas, int height, int width, void *stream);
+int mdt_render_prims(const mdt_render_prim *prims, int n_prims, unsigned char *canvas, int height, int width, void *stream);
+
 /* number of kernel launches issued by this library since load (all entry points) — feeds bench.py's gpu_launches */
 unsigned long long mdt_launch_count(void);
 

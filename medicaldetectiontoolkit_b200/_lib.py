@@ -152,6 +152,9 @@ SIGNATURES = {
     "mdt_petct_normalize_workspace_bytes": (_SZ, [_I64]),
     "mdt_petct_normalize": (_I, [_VP, _VP, _I64, _VP, _VP, _VP, _SZ, _VP]),
     "mdt_toy_images": (_I, [_VP, _I, _I, _I, _I, _I, _VP, _VP, _VP]),
+    "mdt_render_panel_range": (_I, [_VP, _I, _VP, _VP]),
+    "mdt_render_panels": (_I, [_VP, _I, _VP, _VP, _I, _VP, _I, _I, _VP]),
+    "mdt_render_prims": (_I, [_VP, _I, _VP, _I, _I, _VP]),
 }
 
 

@@ -9,8 +9,12 @@ device the calls raise, like the other native ops.
 Dependencies: scikit-learn is never imported.  pandas is imported only to build `test_df` (on first access) and to write or read the
 per-fold `*_test_df.pickle` files, which are the reference's format; the scores themselves need only numpy.
 
-Plotting is not implemented: cf.plot_prediction_histograms and cf.plot_stat_curves are accepted and produce no files, and matplotlib is
-not a dependency.
+Plots: when cf.plot_dir names an existing directory (the reference's runner creates it before training), return_metrics writes the
+reference's files there with plotting.py (rendered on the GPU; matplotlib is not a dependency): with cf.plot_prediction_histograms,
+pred_hist_{fold}_{val|mode}_{level}_cl{cl}.png per class and score level; with cf.plot_stat_curves, {fold}_{mode}_stat_curves_{roc|prc}.png.
+Without one (no plot_dir, None, or a path that is not a directory) it writes nothing.  Documented deviation:
+the reference's plot_stat_curves raises on a patient-level stat whose curve is np.nan (a class with one label value), indexing nan[0];
+here that curve is skipped.
 
 Documented deviation: with cf.scan_det_thresh the reference passes the ROI APs at the thresholds np.arange(0.9, 1, 0.01) to logger.info
 as a stray argument, so they are never printed; here they are formatted into the message.  They are computed at the 'rois' score level
@@ -30,6 +34,7 @@ import numpy as np
 import torch
 
 from . import _lib as L
+from . import plotting
 
 TYPES = ('det_tp', 'det_fp', 'det_fn', 'patient_tn')      # type codes 0..3 of csrc/evaluate.cu
 RECALL_POINTS = np.linspace(.0, 1, 101, endpoint=True)      # compute_roi_ap's R
@@ -258,7 +263,8 @@ class Evaluator():
     # ------------------------------------------------------------------------------------------------------------- the metrics
     def return_metrics(self, monitor_metrics=None):
         """AP / AUC per class and score level (cf.report_score_level) of the stored rows, plus the average foreground ROI AP.
-        Returns (all_stats, monitor_metrics) as the reference does; with monitor_metrics, this epoch's values are appended to it."""
+        Returns (all_stats, monitor_metrics) as the reference does; with monitor_metrics, this epoch's values are appended to it.  Writes the
+        prediction histograms and stat curves cf asks for into cf.plot_dir when that is a directory (see the module docstring)."""
         cf, c = self.cf, self._cols
         classes = list(cf.class_dict.keys())
         folds = _unique_in_order(c['fold'])[0]
@@ -278,6 +284,9 @@ class Evaluator():
             if 'patient' in levels:
                 pat.add_class(cl, cmask, folds if multi_fold else ())
         res = _run_metric_kernels(roi, pat, thresholds)
+        plot_dir = getattr(cf, 'plot_dir', None)
+        if plot_dir is not None and not os.path.isdir(plot_dir):
+            plot_dir = None
 
         all_stats = []
         for cl in classes:
@@ -309,11 +318,15 @@ class Evaluator():
                     monitor_metrics[score_level_name + '_ap'].append(stats_dict['ap'] if stats_dict['ap'] > 0 else None)
                     if score_level == 'patient':
                         monitor_metrics[score_level_name + '_auc'].append(stats_dict['auc'] if stats_dict['auc'] > 0 else None)
+                if plot_dir is not None and cf.plot_prediction_histograms:
+                    self._plot_hist(plot_dir, cl, score_level, codes)
                 all_stats.append(stats_dict)
                 if cf.scan_det_thresh and score_level == 'rois':
                     aps = [roi.ap(res, ('all', cl), 1 + k) for k in range(len(SCAN_THRESHOLDS))]
                     self.logger.info('results from scanning over det_threshs: {}'.format([[i, j] for i, j in zip(SCAN_THRESHOLDS, aps)]))
 
+        if plot_dir is not None and cf.plot_stat_curves:
+            plotting.plot_stat_curves(all_stats, os.path.join(plot_dir, '{}_{}_stat_curves'.format(cf.fold, self.mode)))
         avg_ap = np.mean([d['ap'] for d in all_stats if 'rois' in d['name']])
         all_stats.append({'name': 'average_foreground_roi', 'auc': 0, 'ap': avg_ap})
         if multi_fold:
@@ -324,6 +337,26 @@ class Evaluator():
             if 'val' in self.mode and monitor_metrics[sc].count(monitor_metrics[sc][-1]) > 1 and monitor_metrics[sc][-1] is not None:
                 monitor_metrics[sc][-1] += 1e-6 * np.random.rand()
         return all_stats, monitor_metrics
+
+    def _plot_hist(self, plot_dir, cl, score_level, codes):
+        """the reference's prediction histogram of one class and score level: the ROI rows without patient_tn dummies (with their types), or
+        per patient (sorted pids) the max label and max score"""
+        c = self._cols
+        cmask = c['pred_class'] == cl
+        if score_level == 'rois':
+            spec = cmask & (codes != 3)
+            labels, preds, types = c['class_label'][spec].tolist(), c['pred_score'][spec].tolist(), c['det_type'][spec].tolist()
+        else:
+            idx = np.nonzero(cmask)[0]
+            _, inv = np.unique(c['pid'][idx], return_inverse=True)
+            inv = inv.reshape(-1)
+            n = int(inv.max()) + 1 if idx.size else 0
+            lab, sc = np.full(n, np.iinfo(np.int64).min, np.int64), np.full(n, -np.inf)
+            np.maximum.at(lab, inv, c['class_label'][idx])
+            np.maximum.at(sc, inv, c['pred_score'][idx])
+            labels, preds, types = lab.tolist(), sc.tolist(), None
+        name = 'pred_hist_{}_{}_{}_cl{}'.format(self.cf.fold, 'val' if 'val' in self.mode else self.mode, score_level, cl)
+        plotting.plot_prediction_hist(labels, preds, types, os.path.join(plot_dir, name))
 
     def score_test_df(self, internal_df=True):
         """Writes this fold's rows to <exp_dir>/<fold>_test_df.pickle and its scores to results.txt; once cf.n_cv_splits fold pickles exist,
